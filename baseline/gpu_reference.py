@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """GPU reference of BASELINE.md §3a, measured on the same box as our kernels: the UNMODIFIED reference kernels and
-modules (InternLM/xtuner, installed under ``baseline/_ref`` — git-ignored, never part of this repo's sources, see
-``scripts/install_reference.sh``) at config C2.  BENCH-ONLY: nothing under ``xtuner_b200/`` imports this file.
+modules (InternLM/xtuner, the git-ignored copy under ``oracle/_ref``, see
+``oracle/make_ref.py``) at config C2.  BENCH-ONLY: nothing under ``xtuner_b200/`` imports this file.
 
 Part A, kernel by kernel (what each of our kernels replaces), CUDA-event timed over rotating buffers (> L2):
   * Triton ``m_grouped_gemm`` forward / dX (``xtuner/v1/ops/moe/cuda/triton_kernels/m_grouped_gemm_TMA_triton3_4.py``) and
@@ -15,7 +15,7 @@ Part B: the MoE half of ``MoEDecoderLayer._forward`` (``moe_decoder_layer.py:392
 classes (RMSNorm, MoEGate+GreedyRouter, NaiveDispatcher, MoEBlock) — forward + backward of one layer, eager (the
 reference's ``compile_cfg=False`` mode).
 
-Usage:  python baseline/gpu_reference.py [--out profiles/r02_gpu_reference.json]     (1 GPU; several minutes: ~100 Triton
+Usage:  python baseline/gpu_reference.py [--out FILE]     (1 GPU; several minutes: ~100 Triton
 autotune compilations)
 """
 from __future__ import annotations
@@ -29,7 +29,7 @@ import time
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.path.join(HERE, "_ref")
+REF = os.path.join(os.path.dirname(HERE), "oracle", "_ref")
 C2 = dict(T=8192, H=2048, I=768, E=8, K=2)
 
 
@@ -61,7 +61,7 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     args = ap.parse_args()
     if not os.path.isdir(os.path.join(REF, "xtuner", "v1")):
-        print(json.dumps({"gpu_reference": None, "unavailable": "baseline/_ref is absent (run scripts/install_reference.sh where /root/reference exists)"}))
+        print(json.dumps({"gpu_reference": None, "unavailable": "oracle/_ref is absent (build() places it where a reference checkout is available)"}))
         return
     os.environ.pop("XTUNER_DETERMINISTIC", None)
     import torch

@@ -1,5 +1,5 @@
 /*
- * xtuner_b200.h — C-ABI of the B200-native (sm_100a) MoE hot path for XTuner V1.
+ * xtuner_b200.h — C-ABI of the H100-native (sm_90a) MoE hot path for XTuner V1.
  *
  * Drop-in boundary (SURVEY.md §8b).  Every entry point takes raw DEVICE pointers, plain sizes and a
  * cudaStream_t (passed as void*); no torch types, no allocation inside (workspaces are passed in, sized
@@ -36,7 +36,7 @@ enum xtb_status {
   XTB_OK = 0,
   XTB_ERR_INVALID = 1,     /* bad argument / unsupported shape */
   XTB_ERR_CUDA = 2,        /* CUDA runtime / driver error (message has the string) */
-  XTB_ERR_UNSUPPORTED = 3, /* device is not sm_100 */
+  XTB_ERR_UNSUPPORTED = 3, /* device is not sm_90 */
 };
 
 enum xtb_scoring { XTB_SCORE_SOFTMAX = 0, XTB_SCORE_SIGMOID = 1 };
@@ -44,7 +44,7 @@ enum xtb_scoring { XTB_SCORE_SOFTMAX = 0, XTB_SCORE_SIGMOID = 1 };
 /* ---- library ---------------------------------------------------------------------------------- */
 int xtb_version(void);
 const char* xtb_last_error(void);
-/* Checks that the current device is sm_100 and resolves the driver entry points (TMA descriptors). */
+/* Checks that the current device is sm_90 and resolves the driver entry points (TMA descriptors). */
 int xtb_init(void);
 /* Number of kernels this library has launched since load / last reset (bench.py "gpu_launches"). */
 int64_t xtb_launch_count(void);
@@ -80,7 +80,7 @@ int xtb_router_greedy_dispatch(const float* logits, int T, int E, int K, int sco
                                float scaling, float* router_weights, float* topk_weights, int64_t* topk_ids,
                                int32_t* topk_ids_i32, int64_t* tokens_per_expert, void* dispatch_workspace,
                                xtb_stream_t stream);
-/* a1 + a2 + the index half of a4 in ONE launch (csrc/gate_mma.cu) — what the fused layer calls; bit-equal on a B200 to the two
+/* a1 + a2 + the index half of a4 in ONE launch (csrc/gate_mma.cu) — what the fused layer calls; bit-equal on an H100 to the two
  * calls it stands for when they use the same tensor-core gate (tests/test_gpu_router.py).  Gate logits on
  * the tensor cores (fp32 weight as three bf16 planes, exact products, fp32 accumulation), then the greedy router of
  * xtb_router_greedy_dispatch on the 32-token block that is still in shared memory, then the chunk histograms and their
@@ -98,7 +98,7 @@ int xtb_router_greedy_bwd(const float* router_weights, const float* topk_weights
                           const float* grad_logits_direct, int T, int E, int K, int scoring, int norm_topk_prob,
                           float scaling, float* grad_logits, xtb_stream_t stream);
 
-/* backward of a2 and of a1 in ONE launch — what the fused layer calls; bit-equal on a B200 to xtb_router_greedy_bwd +
+/* backward of a2 and of a1 in ONE launch — what the fused layer calls; bit-equal on an H100 to xtb_router_greedy_bwd +
  * xtb_gate_logits_bwd (tests/test_gpu_router.py): grad_logits is computed per token in the
  * prologue of the gate backward (same formula and order as xtb_router_greedy_bwd) and never written to memory;
  * grad_w / grad_x as xtb_gate_logits_bwd (no bias).  workspace: xtb_gate_logits_bwd_workspace_bytes(T, H, E).
@@ -169,7 +169,7 @@ int xtb_moe_unpermute_bwd(const void* grad_out_bf16, const void* y_fwd_bf16, con
                           xtb_stream_t stream);
 
 /* ---- a6/a7  grouped expert GEMMs: ops/moe/protocol.py:6-12, ops/moe/cuda/group_gemm.py:8-37 ----------
- * tcgen05 (UMMA) kernels, fp32 accumulation in TMEM, bf16 in/out.  tokens_per_expert is a DEVICE int64
+ * wgmma kernels, fp32 accumulation in registers, bf16 in/out.  tokens_per_expert is a DEVICE int64
  * [E] tensor (never read on the host); rows of x are sorted by expert (group e owns rows
  * [cumsum[e-1], cumsum[e]) ).  M_total = rows of x (sum of tokens_per_expert).
  *
@@ -227,7 +227,7 @@ int xtb_moe_dispatch_bwd_rmsnorm(const void* g_xperm_bf16, const int32_t* row_id
 
 /* ==== fp8 tile-wise quantisation (row a15, config 5) ============================================================
  * e4m3, scale = clamp(amax, 1e-12) / 448 (xtuner/v1/float8/float8_utils.py:6-32, fsdp_utils.py:75-116,195-223,
- * triton_kernels/per_tile_quant.py:61-100).  Bit-exact against reference-made golden vectors on a B200
+ * triton_kernels/per_tile_quant.py:61-100).  Bit-exact against reference-made golden vectors on an H100
  * (tests/test_gpu_fp8.py).  Nothing on the bf16 default path calls these; `plugin.install_fp8_cast()` rebinds the
  * reference's FSDP fp8 all-gather cast (`WeightWithDynamicTilewiseFloat8CastTensor.fsdp_pre_all_gather`,
  * fsdp_utils.py:379-409) and its scale precompute to them.  There is no fp8 grouped GEMM here yet. */

@@ -3,7 +3,7 @@ imports it).  Each method takes exactly the arguments of the header's declaratio
 handle that is ignored) and computes the documented result with plain torch-CPU / oracle arithmetic on the memory the
 addresses point at.  It lets the CPU suite drive the shipped host orchestration above the boundary — the single-node
 fused layer of ``xtuner_b200/fused.py``: buffer shapes, argument order, the backward chain — which otherwise only
-runs on a B200.  It is NOT bit-compatible with the kernels in every rounding (tests use bf16-level tolerances) and
+runs on an H100.  It is NOT bit-compatible with the kernels in every rounding (tests use bf16-level tolerances) and
 implements only the entry points that orchestration uses."""
 from __future__ import annotations
 

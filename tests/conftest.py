@@ -11,7 +11,7 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -25,16 +25,32 @@ def pytest_collection_modifyitems(config, items):
         has_cuda = False
     if has_cuda:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200); run with -m gpu on the GPU box")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100); run with -m gpu")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)
 
 
 def load_golden(name):
+    """``<name>.pt``, or for a large fixture ``<name>.part<i>.pt``: lists of (key path, value) merged into one dict."""
+    import glob
+
     import torch
 
-    return torch.load(os.path.join(GOLDEN_DIR, name + ".pt"), weights_only=False)
+    whole = os.path.join(GOLDEN_DIR, name + ".pt")
+    if os.path.exists(whole):
+        return torch.load(whole, weights_only=False)
+    parts = sorted(glob.glob(os.path.join(GOLDEN_DIR, name + ".part*.pt")))
+    if not parts:
+        raise FileNotFoundError(whole)
+    out = {}
+    for part in parts:
+        for path, value in torch.load(part, weights_only=False):
+            d = out
+            for key in path[:-1]:
+                d = d.setdefault(key, {})
+            d[path[-1]] = value
+    return out
 
 
 @pytest.fixture

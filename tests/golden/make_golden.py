@@ -1,11 +1,12 @@
 """Generate golden input/output vectors for the MoE hot path by running the REFERENCE'S OWN CODE
-(imported from /root/reference through ``ref_shim``) on CPU with seeded inputs.
+(imported through ``ref_shim``) on CPU with seeded inputs.
 
-Run in the authoring container only (the GPU box has no /root/reference):
+Run where the reference tree is available (``XTUNER_REFERENCE_ROOT``):
 
     python tests/golden/make_golden.py
 
-Outputs: ``tests/golden/*.pt`` (small, committed).  Each fixture is a flat ``dict[str, Tensor|int|float|str]``.
+Outputs: ``tests/golden/*.pt`` (small, committed).  Each fixture is a flat ``dict[str, Tensor|int|float|str]``; one above
+~0.9 MB is written as ``<name>.part<i>.pt`` (``tests/conftest.py::load_golden`` merges the parts).
 The reference objects exercised are named in each section; nothing here comes from ``oracle/``.
 Inputs are tie-free by construction (fp32 logits from a continuous RNG; SURVEY.md §7 "bit-exact routing").
 """
@@ -37,7 +38,34 @@ def save(name: str, obj: dict) -> None:
     obj = {k: (v.detach().clone() if isinstance(v, torch.Tensor) else v) for k, v in obj.items()}
     path = os.path.join(HERE, name + ".pt")
     torch.save(obj, path)
+    if os.path.getsize(path) > PART_BYTES:
+        os.remove(path)
+        save_parts(name, obj)
+        return
     print(f"wrote {path}  ({os.path.getsize(path) / 1024:.1f} KiB)")
+
+
+PART_BYTES = 900_000
+
+
+def save_parts(name: str, obj: dict) -> None:
+    """``<name>.part<i>.pt``: lists of (key path, value), each file below PART_BYTES."""
+    import io
+
+    def flatten(d, pre=()):
+        for k, v in d.items():
+            yield from flatten(v, pre + (k,)) if isinstance(v, dict) else [(pre + (k,), v)]
+
+    parts, cur = [[]], 0
+    for path, v in flatten(obj):
+        buf = io.BytesIO()
+        torch.save(v, buf)
+        if cur + buf.tell() > PART_BYTES and parts[-1]:
+            parts, cur = parts + [[]], 0
+        parts[-1].append((path, v))
+        cur += buf.tell()
+    for i, part in enumerate(parts):
+        torch.save(part, os.path.join(HERE, f"{name}.part{i}.pt"))
 
 
 def run_naive_dispatcher(disp, hidden_states, topk_ids, topk_weights, experts):

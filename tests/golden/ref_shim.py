@@ -17,7 +17,8 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("XTUNER_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("XTUNER_REFERENCE_ROOT") or os.path.join(
+    os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "oracle", "_ref")  # oracle/make_ref.py
 
 
 def reference_available() -> bool:

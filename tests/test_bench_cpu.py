@@ -36,9 +36,6 @@ def test_summarize_profile_rooflines():
     assert abs(disp["gather_only_GBs"] - 100794368 / 0.021e-3 / 1e9) < 1e-3
     assert kus["xtb_group_gemm_nn"] == 70.0 and kus["xtb_moe_combine"] == 29.0
     json.dumps({"roofline": roof, "roofline_dispatch": disp})  # serialisable
-    if os.path.exists(os.path.join(ROOT, "profiles", "ncu_traffic.json")):
-        assert roof["traffic"] and roof["traffic"] > 5e7
-        assert disp["traffic"]["gather"] and disp["traffic"]["combine"]
 
 
 def test_dispatch_roofline_with_fused_gate_route():

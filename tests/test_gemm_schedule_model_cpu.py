@@ -1,13 +1,13 @@
-"""Model of the persistent tile schedule of ``group_gemm2_kernel`` (csrc/group_gemm.cu): restates the device-side tile scan
-(``s_tile_start`` from ``tokens_per_expert``) and ``decode(tile)`` and checks, for ragged expert sizes, that every 256-row x
-256-column piece of the output is produced exactly once and that each cluster sees its tiles in non-decreasing order (the
-monotone expert search relies on it).  Also records the wave quantisation of the C2 shapes — the open item of DESIGN.md §4
-(a split of the last wave into 256x128 halves was tried on hardware and bought nothing: profiles/r02_ab_switches.txt)."""
+"""Model of the persistent tile schedule of ``group_gemm_kernel`` (csrc/group_gemm.cu): restates the device-side tile scan
+(``s_tile_start`` from ``tokens_per_expert``) and ``decode(tile)`` and checks, for ragged expert sizes, that every 128-row x
+BLOCK_N-column piece of the output is produced exactly once and that each CTA sees its tiles in non-decreasing order (the
+monotone expert search relies on it).  Also records the wave quantisation of the C2 shapes on the 132 SMs of an H100."""
 import random
 
 import pytest
 
-BM = 256
+BM = 128
+SMS = 132  # persistent CTAs of the kernel on an H100 ("cluster" below: one CTA)
 
 
 def schedule(counts, n_tiles, n_clusters, mode_tn=False, m_out_tiles=0):
@@ -42,7 +42,7 @@ def schedule(counts, n_tiles, n_clusters, mode_tn=False, m_out_tiles=0):
     return total_tiles, per_cluster
 
 
-@pytest.mark.parametrize("n_tiles,n_clusters", [(6, 74), (3, 74), (8, 74), (6, 5), (1, 3)])
+@pytest.mark.parametrize("n_tiles,n_clusters", [(6, SMS), (3, SMS), (8, SMS), (6, 5), (1, 3)])
 def test_every_output_tile_is_produced_once(n_tiles, n_clusters):
     rng = random.Random(n_tiles * 100 + n_clusters)
     for trial in range(20):
@@ -61,16 +61,17 @@ def test_every_output_tile_is_produced_once(n_tiles, n_clusters):
 
 
 def test_c2_wave_quantisation():
-    """At C2 (8 experts x 2048 rows, 74 clusters) four of the six products run 384 or 192 pair-tiles: 86 % wave efficiency."""
+    """At C2 (8 experts x 2048 rows = 16 row blocks each, 132 CTAs, 256-column tiles) every product runs a multiple of 384
+    tiles: 2.9 waves of work per 3 waves, 97 % wave efficiency."""
     uniform = [2048] * 8
-    waves = lambda tiles: -(-tiles // 74)
-    for n_tiles, tiles in [(6, 384), (3, 192), (8, 512)]:  # w13 NT (N=1536), dX of w2 (N=768), w2 NT / dX of w13 (N=2048)
-        total, _ = schedule(uniform, n_tiles, 74)
+    waves = lambda tiles: -(-tiles // SMS)  # noqa: E731
+    for n_tiles, tiles in [(6, 768), (3, 384), (8, 1024)]:  # w13 NT (I=768: 128 features per tile), dX of w2 (768), w2 NT / dX of w13 (2048)
+        total, _ = schedule(uniform, n_tiles, SMS)
         assert total == tiles
-    assert round(384 / 74 / waves(384), 3) == 0.865 and round(192 / 74 / waves(192), 3) == 0.865
-    assert round(512 / 74 / waves(512), 3) == 0.988
-    total, _ = schedule(uniform, 8, 74, mode_tn=True, m_out_tiles=6)  # dW13: 8 experts x 6 x 8
-    assert total == 384
+    assert round(384 / SMS / waves(384), 3) == 0.97 and round(768 / SMS / waves(768), 3) == 0.97
+    assert round(1024 / SMS / waves(1024), 3) == 0.97
+    total, _ = schedule(uniform, 8, SMS, mode_tn=True, m_out_tiles=12)  # dW13: 8 experts x 12 x 8
+    assert total == 768
 
 
 def schedule_tn_pair(E, geo_a, geo_b, n_clusters):
@@ -92,7 +93,7 @@ def schedule_tn_pair(E, geo_a, geo_b, n_clusters):
     return tiles0 + tiles1, [[decode(t) for t in range(c, tiles0 + tiles1, n_clusters)] for c in range(n_clusters)]
 
 
-@pytest.mark.parametrize("E,geo_a,geo_b,n_clusters", [(8, (8, 3), (6, 8), 74), (4, (4, 2), (4, 4), 74), (5, (1, 2), (2, 1), 3)])
+@pytest.mark.parametrize("E,geo_a,geo_b,n_clusters", [(8, (16, 3), (12, 8), SMS), (4, (4, 2), (4, 4), SMS), (5, (1, 2), (2, 1), 3)])
 def test_tn_pair_tile_list_covers_both_products_once(E, geo_a, geo_b, n_clusters):
     total, per_cluster = schedule_tn_pair(E, geo_a, geo_b, n_clusters)
     seen = [t for seq in per_cluster for t in seq]
@@ -103,9 +104,15 @@ def test_tn_pair_tile_list_covers_both_products_once(E, geo_a, geo_b, n_clusters
     assert max(sizes) - min(sizes) <= 1
 
 
-def test_tn_pair_fills_the_last_wave_at_c2():
-    """dW2 (8 x 8 x 3 = 192 tiles) and dW13 (8 x 6 x 8 = 384 tiles) alone: 3 + 6 waves over 74 clusters for 2.6 + 5.2 waves of
-    work; as one tile list: 576 tiles = 8 waves (profiles/r02_kbench.txt: 124 us against 48 + 87 us)."""
-    waves = lambda tiles: -(-tiles // 74)  # noqa: E731
-    total, _ = schedule_tn_pair(8, (8, 3), (6, 8), 74)
-    assert total == 576 and waves(192) + waves(384) == 9 and waves(total) == 8
+def test_tn_pair_never_needs_more_waves_than_two_launches():
+    """One tile list over both weight gradients never takes more waves than the two launches, and saves one whenever the
+    two last waves fit into one.  At C2 on 132 CTAs (384 + 768 tiles) both ways take 9 waves."""
+    waves = lambda tiles: -(-tiles // SMS)  # noqa: E731
+    for E, geo_a, geo_b in [(8, (16, 3), (12, 8)), (8, (8, 3), (6, 8)), (4, (4, 2), (4, 4)), (3, (2, 2), (1, 5))]:
+        ta, tb = E * geo_a[0] * geo_a[1], E * geo_b[0] * geo_b[1]
+        total, _ = schedule_tn_pair(E, geo_a, geo_b, SMS)
+        assert total == ta + tb and waves(total) <= waves(ta) + waves(tb)
+        if (ta % SMS) and (tb % SMS) and (ta % SMS) + (tb % SMS) <= SMS:
+            assert waves(total) == waves(ta) + waves(tb) - 1
+    total, _ = schedule_tn_pair(8, (16, 3), (12, 8), SMS)
+    assert total == 1152 and waves(384) + waves(768) == 9 and waves(total) == 9

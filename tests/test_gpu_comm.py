@@ -35,7 +35,7 @@ def test_fsdp2_custom_collectives():
 @pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
 def test_ep_dispatcher_gpu():
     """ep > 1 dispatchers (NCCL all-to-all and the device-driven peer exchange) against ep = 1, forward and backward, incl.
-    async_op=True — green at 2 and at 8 B200s (profiles/r02_n8_log.txt)."""
+    async_op=True.  Not run on H100 (needs two GPUs)."""
     n = min(torch.cuda.device_count(), int(os.environ.get("XTB_TEST_WORLD", "2")))
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={n}", "--master-addr", "127.0.0.1",
            "--master-port", "29535", os.path.join(ROOT, "tests", "multigpu", "ep_worker.py")]

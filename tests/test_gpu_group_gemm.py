@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 grouped GEMMs (forward NT, dX NN, dW TN) against the oracle's per-expert
+"""GPU parity of the wgmma grouped GEMMs (forward NT, dX NN, dW TN) against the oracle's per-expert
 loop (tests/ops/test_grouped_gemm_triton.py:6-23 semantics) — small ragged cases on the CPU oracle, full
 config sizes against a per-expert cuBLAS loop on the same GPU (fp32-accumulate yardstick).
 Tolerance: the reference's own (rtol=atol=1e-2, tests/ops/test_grouped_gemm_triton.py:62-64) or tighter."""
@@ -32,7 +32,7 @@ def _loop(x, w, counts):
 @pytest.mark.parametrize(
     "E,M,N,Kd,empty",
     [(4, 300, 128, 128, ()), (8, 1000, 256, 128, (2,)), (8, 77, 128, 256, (0, 7)), (3, 129, 384, 192 + 64, ()), (1, 128, 128, 128, ()),
-     # shapes that take the CTA-pair (256x256-tile) kernel
+     # shapes that take the 256-column tiles
      (4, 700, 256, 256, ()), (8, 1000, 512, 256, (2,)), (3, 100, 256, 512, (1,)), (2, 513, 768, 256, ())],
 )
 def test_group_gemm_small_vs_cpu_oracle(E, M, N, Kd, empty):

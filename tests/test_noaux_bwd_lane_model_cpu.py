@@ -1,7 +1,7 @@
 """Lane-level model of ``router_noaux_bwd_kernel<LPT, VPL>`` (csrc/route.cu): LPT lanes per token, each holding VPL
 consecutive experts, xor-shuffle reductions for the row sums, the group mask read back from ``router_weights != 0``, the
 top-k gradient scattered by id.  Restates the kernel's per-lane arithmetic and checks it against the reference-made
-gradient fixture — the kernel itself is covered on the B200 by tests/test_gpu_router.py (noaux backward vs the same fixture)."""
+gradient fixture — the kernel itself is covered on the GPU by tests/test_gpu_router.py (noaux backward vs the same fixture)."""
 import numpy as np
 import pytest
 import torch

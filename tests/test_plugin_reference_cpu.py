@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import ref_shim  # noqa: E402
 
-pytestmark = pytest.mark.skipif(not ref_shim.reference_available(), reason="reference tree not mounted")
+pytestmark = pytest.mark.skipif(not ref_shim.reference_available(), reason="no reference checkout found")
 
 
 def _install_cpu_kernel_standins(monkeypatch):

@@ -1,5 +1,5 @@
-"""GPU worker: the UNMODIFIED reference MoE model (installed under baseline/_ref, see scripts/install_reference.sh) on a
-B200 — first on the reference's own GPU path (Triton grouped GEMM, torch-fallback permute/unpermute), then with
+"""GPU worker: the UNMODIFIED reference MoE model (the copy under oracle/_ref, see oracle/make_ref.py) on an
+H100 — first on the reference's own GPU path (Triton grouped GEMM, torch-fallback permute/unpermute), then with
 ``xtuner_b200.plugin.convert_model`` (per-op classes) and ``convert_model(fused=True)`` (one autograd node per MoE half).
 The recipe is the reference's ``tests/model/test_moe.py:57-148`` (tiny random-init MoE, same batch through two
 dispatcher implementations).  Prints one JSON line; tests/test_gpu_reference_plugin.py asserts on it."""
@@ -9,7 +9,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def main():

@@ -1,4 +1,4 @@
-"""xtuner_b200 — B200-native (sm_100a) drop-in for XTuner V1's data-parallel MoE training hot path.
+"""xtuner_b200 — H100-native (sm_90a) drop-in for XTuner V1's data-parallel MoE training hot path.
 
 Host code is thin Python over a C-ABI CUDA library (``include/xtuner_b200.h``).  Importing this package
 does not need a GPU; calling any compute op does (there is no CPU fallback)."""

@@ -158,7 +158,7 @@ _initialised = False
 
 
 def ensure_init() -> ctypes.CDLL:
-    """Load + xtb_init() (checks for an sm_100 device).  Raises if there is no usable GPU."""
+    """Load + xtb_init() (checks for an sm_90 device).  Raises if there is no usable GPU."""
     global _initialised
     lib = load()
     if not _initialised:

@@ -194,8 +194,7 @@ __global__ void __launch_bounds__(256) allreduce_pull_f32_kernel(const float4* c
 }
 
 // CTAs of an exchange kernel: 2 per SM.  The kernels run under the grouped GEMMs of the neighbouring layer; capping the
-// grid lower (32 / 64 CTAs) was measured at N=2 (profiles/r02a_comm_n2.json): the all-gather takes 295 / 158 us instead of
-// 84 us and the step gets slower, because the exchange then outlasts the compute it hides under.
+// grid lower makes the exchange outlast the compute it hides under.  The grid size has not been measured on H100.
 static int comm_blocks(long long n_vec) {
   const long long want = (n_vec + 256 * 8 - 1) / (256 * 8);
   return (int)max(1ll, min(want, (long long)sm_count() * 2));

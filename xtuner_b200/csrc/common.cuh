@@ -1,4 +1,4 @@
-// Shared host/device helpers for the sm_100a kernels behind include/xtuner_b200.h.
+// Shared host/device helpers for the sm_90a kernels behind include/xtuner_b200.h.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
 // fp8 (e4m3) tile-wise quantisation kernels for the fp8 expert path (SURVEY.md §8a row a15, config 5).
-// Bit-exact on a B200 against reference-made golden vectors and the oracle (tests/test_gpu_fp8.py; oracle/moe_oracle.py:
+// Bit-exact on an H100 against reference-made golden vectors and the oracle (tests/test_gpu_fp8.py; oracle/moe_oracle.py:
 // per_tile_quant, per_block_fp8_scales, cast_to_per_block_fp8).  Nothing on the bf16 default path calls them;
 // plugin.install_fp8_cast() rebinds the reference's fp8 FSDP all-gather cast and scale precompute to them.
 //

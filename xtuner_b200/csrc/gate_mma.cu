@@ -1,6 +1,6 @@
 // a1 (MoEGate.forward, moe_decoder_layer.py:120-141) on the tensor cores, and the one-launch gate + greedy router +
-// dispatch bucketing built on it (xtb_gate_route_dispatch: the default of the fused layer for E <= 8, 27.9 us against
-// 22.0 + 11.8 us for the two calls at C2, profiles/r02_ab_switches.txt).  The stand-alone kernel (XTB_GATE_V=2 inside
+// dispatch bucketing built on it (xtb_gate_route_dispatch: the default of the fused layer for E <= 8; fused against
+// two calls has not been measured on H100).  The stand-alone kernel (XTB_GATE_V=2 inside
 // xtb_gate_logits) is what the GPU test compares the fused launch with, bit for bit
 // (tests/test_gpu_router.py::test_gate_route_dispatch_equals_two_calls); fragment mapping modelled lane by lane on CPU
 // (tests/test_gate_mma_mapping_cpu.py).
@@ -12,7 +12,7 @@
 //   * x (bf16, exact) streams from global memory straight into A fragments of mma.sync.m16n8k16 (bf16 x bf16
 //     products are exact in fp32; fp32 accumulation),
 // so per 32 columns a warp issues 2 x LDG.128, 3 x LDS.128 (conflict free) and 6 HMMAs for 16 tokens.
-// This is HBM/L2-streaming work, not GEMM-shaped work: mma.sync (not tcgen05) is the right tool — N = 8.
+// This is HBM/L2-streaming work, not GEMM-shaped work: mma.sync (not wgmma) is the right tool — N = 8.
 //
 // K ordering trick: inside a 32-column block, lane (g = lane/4, t = lane%4) owns columns t*8 .. t*8+7 of rows g and
 // g+8.  MMA step s in {0,1} takes the lane's elements 4s..4s+3 as logical k = {2t, 2t+1, 2t+8, 2t+9}.  A and B use the

@@ -25,17 +25,17 @@ int fail(int code, const char* fmt, ...) {
 }
 
 bool pdl_enabled() {
-  static const bool on = !(getenv("XTB_PDL") && atoi(getenv("XTB_PDL")) == 0);  // default on (-1 % step, profiles/r02)
+  static const bool on = !(getenv("XTB_PDL") && atoi(getenv("XTB_PDL")) == 0);  // default on
   return on;
 }
 
 int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -109,8 +109,8 @@ int xtb_init(void) {
   XTB_CUDA(cudaGetDevice(&dev));
   XTB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   XTB_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  if (major != 10)
-    return xtb::fail(XTB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only", dev,
+  if (major != 9)
+    return xtb::fail(XTB_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", dev,
                      major, minor);
   return xtb_tma_init_();
 }

@@ -405,8 +405,7 @@ __device__ __forceinline__ void swiglu_bwd_vec(const uint4& g, const uint4& u, c
   o_u = make_uint4(o2[0], o2[1], o2[2], o2[3]);
 }
 
-// Round 1's kernel was instruction-bound (ncu: sm__throughput 67-70 %, DRAM 33-39 %): a 64-bit divide per thread to find
-// its row and one 16-byte vector per thread (30-33 us at C2; this one 26.8 us, profiles/r02_kbench.txt).  A block owns
+// A 64-bit divide per thread to find its row, with one 16-byte vector per thread, is instruction-bound.  A block owns
 // kSwRows consecutive rows, the row of a vector comes from a
 // 32-bit multiply-high with a host-made reciprocal, and every thread keeps two vectors' loads in flight.
 constexpr int kSwRows = 8;
@@ -490,8 +489,8 @@ static int permute_impl(const void* x, const int32_t* ids, int T, int K, int E, 
     const size_t smem = (size_t)(kChunkTokens + kSubTokens) * K * sizeof(int);
     const int n_sub = (T + kSubTokens - 1) / kSubTokens;
     const int row_vec = (int)(row_bytes / 16);
-    // rows through shared memory with the bulk-copy engine (default; same speed as the register-staged kernel at C2,
-    // profiles/r02_ab_switches.txt).  XTB_PERMUTE_BULK=0 or rows too long for 8 staged rows: the register-staged kernel.
+    // rows through shared memory with the bulk-copy engine (default; not compared with the register-staged kernel on
+    // H100).  XTB_PERMUTE_BULK=0 or rows too long for 8 staged rows: the register-staged kernel.
     static const bool bulk = !(getenv("XTB_PERMUTE_BULK") && atoi(getenv("XTB_PERMUTE_BULK")) == 0);
     const size_t smem_bulk = (size_t)kSubTokens * row_bytes + kSubTokens * sizeof(uint64_t) + smem;
     if (copy && bulk && smem_bulk <= 200 * 1024) {

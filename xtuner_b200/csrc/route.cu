@@ -165,16 +165,19 @@ __global__ void __launch_bounds__(256) sgemm_strided_kernel(const TA* __restrict
 // [n_blocks, E, H] workspace and reduced (deterministically) by a second kernel.
 // =====================================================================================================
 // The next batch of U token rows is requested before the current one is consumed, so the block's loop is bound by
-// max(load latency, FMA issue) instead of their sum (36.4 -> 34.3 us at C2, profiles/r02_ab_switches.txt).
+// max(load latency, FMA issue) instead of their sum.
 // The streaming part is shared by the plain kernel (grad_logits read from global memory) and the variant that computes
 // them in its prologue from the router's saved tensors (router_gate_bwd_kernel).
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+
 template <int E_MAX>
 __device__ __forceinline__ void gate_bwd_main(const float* __restrict__ s_gl, const __nv_bfloat16* __restrict__ x,
                                               const float* __restrict__ w, float* __restrict__ partial_gw,
                                               __nv_bfloat16* __restrict__ gx, int H, int E, int t_begin, int t_end) {
   // 4 columns per thread (512 threads cover H = 2048): half the accumulators per thread of the 8-column version, so twice
-  // the warps fit next to each other and hide the row loads; the 16 FMAs per element are issued as packed pairs
-  // (fma.rn.f32x2: two IEEE fmas per instruction, same bits as fmaf in the same order).
+  // the warps fit next to each other and hide the row loads.
   for (int h = threadIdx.x * 4; h < H; h += blockDim.x * 4) {
     float2 wr[E_MAX][2];
     float2 acc[E_MAX][2];
@@ -218,10 +221,10 @@ __device__ __forceinline__ void gate_bwd_main(const float* __restrict__ s_gl, co
           for (int i = 0; i < 4; ++i) {
             const int e = e4 * 4 + i;
             const float2 g2 = make_float2(ge[i], ge[i]);
-            g0 = __ffma2_rn(g2, wr[e][0], g0);
-            g1 = __ffma2_rn(g2, wr[e][1], g1);
-            acc[e][0] = __ffma2_rn(g2, xv0, acc[e][0]);
-            acc[e][1] = __ffma2_rn(g2, xv1, acc[e][1]);
+            g0 = fma2(g2, wr[e][0], g0);
+            g1 = fma2(g2, wr[e][1], g1);
+            acc[e][0] = fma2(g2, xv0, acc[e][0]);
+            acc[e][1] = fma2(g2, xv1, acc[e][1]);
           }
         }
         uint2 o;

@@ -1,7 +1,8 @@
-// Thin inline-PTX wrappers for the sm_100a features the grouped GEMM uses: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / fences) and UMMA descriptors.
-// Bit layouts follow the PTX ISA "tcgen05 matrix descriptor / instruction descriptor" tables
-// (cross-checked against cute/arch/mma_sm100_desc.hpp shipped in this image).
+// (The file keeps the name it had when the project targeted sm_100a.)
+// Thin inline-PTX wrappers for the sm_90a features the grouped GEMM uses: mbarrier, TMA
+// (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait), setmaxnreg and the wgmma
+// shared-memory matrix descriptor.  Bit layouts follow the PTX ISA "warpgroup-level matrix
+// shared memory layout / matrix descriptor" tables.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -41,76 +42,19 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Blocking wait with a watchdog: a protocol bug traps (-> CUDA error on the host) instead of hanging
-// the GPU until an external timeout kills the process.
+// the GPU until an external timeout kills the process.  No printf here: a function call between two wgmma
+// groups makes ptxas serialise the wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000ll) {  // ~2 s at 2 GHz
-      printf("xtuner_b200: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
-  }
-}
-
-// ---- cluster helpers (CTA pairs) ------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster.
-// Default (.release.cta) semantics on purpose: the cluster-scope forms compile to MEMBAR.ALL.GPU on the
-// arrive and CCTL.IVALL (L1 invalidate) on every wait, which serialised the pipeline at ~1 us per k-block.
-// What crosses CTAs here is shared memory written by TMA / fenced with fence.proxy.async and TMEM reads
-// completed with tcgen05.wait::ld — none of it lives in L1 or needs a GPU-scope fence.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n"
-      ".reg .b32 ra;\n"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// wait for arrivals that may come from the peer CTA (cluster-scope acquire), with the same watchdog
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait_cluster(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if (clock64() - t0 > 4000000000ll) {
-      printf("xtuner_b200: cluster mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000ll) __trap();  // ~2 s at 2 GHz
   }
 }
 
 // ---- proxies / fences ---------------------------------------------------------------------------------
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---- TMA ------------------------------------------------------------------------------------------------
@@ -122,20 +66,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// CTA-pair load: the bytes land in THIS CTA's shared memory but complete_tx is signalled on the mbarrier at
-// the same offset in the LEADER CTA of the pair (cluster rank 0), so the MMA issuer waits on a single barrier.
-__device__ __forceinline__ void tma_load_2d_signal_leader(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0,
-                                                          int c1, uint32_t leader = 0) {
-  asm volatile(
-      "{\n"
-      ".reg .b32 lb;\n"
-      "mapa.shared::cluster.u32 lb, %2, %5;\n"
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [lb];\n"
-      "}\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(leader)
       : "memory");
 }
 
@@ -153,104 +83,76 @@ __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bu
 // ... have completed entirely (global writes performed)
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- TMEM allocation ----------------------------------------------------------------------------------
-// Must be executed by one full warp; the same warp deallocates.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// CTA-pair (cta_group::2) variants: executed by the same warp index in BOTH CTAs of the pair.
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ---- UMMA descriptors -----------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle, descriptor version 1 (sm_100).
+// ---- wgmma ------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor, 128-byte swizzle.
 //   bits [0,14)  start address >> 4        bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride-dim byte offset >> 4     bits [46,48) version = 1     bits [61,64) layout (2 = SW128)
+//   bits [32,46) stride-dim byte offset >> 4     bits [62,64) layout (1 = 128-byte swizzle)
+// K-major: 8-row groups `sbo` bytes apart (lbo unused).  MN-major: 64-element MN atoms `lbo`, 8-k groups `sbo` apart.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 accumulate.
-//   [4,6) c_format=1 (f32)  [7,10) a_format=1 (bf16)  [10,13) b_format=1 (bf16)
-//   [15] a_major (0=K,1=MN)  [16] b_major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16_f32(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most N of this warpgroup's committed wgmma groups are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// pins the accumulator registers around an asynchronous wgmma
+template <int N>
+__device__ __forceinline__ void fence_accumulator(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS));
+}
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS));
+}
+// named barrier over `threads` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64 x N, registers of one warpgroup] (+)= A[smem, 64 x 16] * B[smem, 16 x N].  TNSP = 1: MN-major operand.  Thread t
+// holds, per 8-column chunk j, d[4j + {0,1}] = row 16 (t / 32) + (t % 32) / 4, columns 8j + 2 (t % 4) + {0,1}; d[4j + {2,3}]: row + 8.
+#define XTB_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define XTB_D64(i) XTB_D8(i), XTB_D8(i + 8), XTB_D8(i + 16), XTB_D8(i + 24), XTB_D8(i + 32), XTB_D8(i + 40), XTB_D8(i + 48), XTB_D8(i + 56)
+#define XTB_R16(a, b, c, d, e, f, g, h, i, j, k, l, m, n, o, p) \
+  "%" #a ",%" #b ",%" #c ",%" #d ",%" #e ",%" #f ",%" #g ",%" #h ",%" #i ",%" #j ",%" #k ",%" #l ",%" #m ",%" #n ",%" #o ",%" #p
+#define XTB_R64_0 XTB_R16(0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15) "," XTB_R16(16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31) "," \
+  XTB_R16(32, 33, 34, 35, 36, 37, 38, 39, 40, 41, 42, 43, 44, 45, 46, 47) "," XTB_R16(48, 49, 50, 51, 52, 53, 54, 55, 56, 57, 58, 59, 60, 61, 62, 63)
+#define XTB_R64_1 XTB_R16(64, 65, 66, 67, 68, 69, 70, 71, 72, 73, 74, 75, 76, 77, 78, 79) "," XTB_R16(80, 81, 82, 83, 84, 85, 86, 87, 88, 89, 90, 91, 92, 93, 94, 95) "," \
+  XTB_R16(96, 97, 98, 99, 100, 101, 102, 103, 104, 105, 106, 107, 108, 109, 110, 111) "," XTB_R16(112, 113, 114, 115, 116, 117, 118, 119, 120, 121, 122, 123, 124, 125, 126, 127)
+template <int TNSP_A, int TNSP_B>
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {" XTB_R64_0 "}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+      : XTB_D64(0)
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TNSP_A), "n"(TNSP_B));
 }
-// Arrive on an mbarrier once all tcgen05 ops previously issued by this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// CTA-pair MMA: D (256 x N, split 128 rows per CTA) (+)= A (128 rows per CTA) * B (N/2 rows per CTA).
-// Issued by one thread of the LEADER CTA; the descriptors are applied at the same smem offsets in both CTAs.
-__device__ __forceinline__ void umma_bf16_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                               uint32_t accumulate) {
+template <int TNSP_A, int TNSP_B>
+__device__ __forceinline__ void wgmma_m64n256k16_bf16(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {" XTB_R64_0 "," XTB_R64_1 "}, %128, %129, p, 1, 1, %131, %132;\n}\n"
+      : XTB_D64(0), XTB_D64(64)
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TNSP_A), "n"(TNSP_B));
 }
-// commit that arrives on the barrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive 32-bit columns (thread i of the warp gets lane base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+#undef XTB_D8
+#undef XTB_D64
+#undef XTB_R16
+#undef XTB_R64_0
+#undef XTB_R64_1
 
 }  // namespace ptx
 }  // namespace xtb

@@ -1,5 +1,5 @@
 """``FusedDispatcher``: the six-phase dispatcher protocol of the reference
-(``xtuner/v1/module/dispatcher/base.py:86-176``) for ep=1, backed by the sm_100a dispatch/combine kernels.
+(``xtuner/v1/module/dispatcher/base.py:86-176``) for ep=1, backed by the sm_90a dispatch/combine kernels.
 
 Same keyword-only methods and TypedDict results as ``NaiveDispatcher`` (``base.py:222-539``); the real
 work is in ``dispatch_postprocess`` (bucket + gather, which also yields ``tokens_per_expert`` from the

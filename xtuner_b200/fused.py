@@ -9,7 +9,7 @@ backward  combine-bwd -> dX/dW grouped GEMMs (w2) -> SwiGLU-bwd -> dX/dW grouped
           -> router-bwd (three gradient routes) -> gate-bwd -> dispatch-bwd fused with the gate-grad add
 
 One Python frame and ~20 kernel launches per layer instead of ~40 dispatcher/custom-op calls: the path is
-launch-bound in eager mode otherwise (profiles/r01a).  Numerics are identical to composing
+launch-bound in eager mode otherwise.  Numerics are identical to composing
 ``xtuner_b200.ops`` (same kernels); the per-op bf16 roundings of the reference are kept (see kernel notes).
 """
 from __future__ import annotations
@@ -24,11 +24,11 @@ from . import _capi, ops
 from ._capi import check, current_stream, ptr
 from .router import SCORING
 
-# ---- fused entry points that won their A/B on hardware (profiles/r02_ab_switches.txt); the env variables only exist so the
+# ---- fused entry points (their A/B against the separate calls has not been repeated on H100); the env variables only exist so the
 # parity tests can still compare each fused kernel with the separate calls it replaces -----------------------------------
 # xtb_gate_route_dispatch : gate (tensor cores) + greedy router + dispatch bucketing in one launch (E <= 8, H % 128 == 0,
-#                           H <= 4096): 27.9 us against 22.0 + 11.8 us for the two calls at C2
-# xtb_router_gate_bwd     : router backward in the prologue of the gate backward (E <= 8): 39.4 us against 36.4 + 9.7 us
+#                           H <= 4096)
+# xtb_router_gate_bwd     : router backward in the prologue of the gate backward (E <= 8)
 GATE_ROUTE_FUSED = os.environ.get("XTB_GATE_ROUTE_FUSED", "1") == "1"
 ROUTER_GATE_BWD_FUSED = os.environ.get("XTB_ROUTER_GATE_BWD_FUSED", "1") == "1"
 
@@ -198,9 +198,8 @@ class FusedMoEBlockFunction(torch.autograd.Function):
         x = torch.empty((T, H), dtype=bf, device=dev)
         rstd = torch.empty((T,), dtype=f32, device=dev)
         logits = torch.empty((T, E), dtype=f32, device=dev)
-        # the norm as its own streaming kernel: folding the gate into it (xtb_rmsnorm_gate with gate_w) measured slower twice
-        # (CUDA-core version profiles/r01c, tensor-core version profiles/r02_ab_switches.txt: 36.6 us against 19.4 + 22.0 and
-        # against the gate+route kernel below)
+        # the norm as its own streaming kernel: folding the gate into it (xtb_rmsnorm_gate with gate_w) is not used by
+        # the fused layer (not measured on H100)
         route_fused = _gate_route_ok(H, E, K)
         _k(lib, "xtb_rmsnorm_gate", ptr(h), ptr(norm_w), None, float(eps), T, H, E, ptr(x), ptr(rstd), None, st)
         rw = torch.empty((T, E), dtype=f32, device=dev)

@@ -1,5 +1,5 @@
 """Host-side mirror of the reference's MoE op protocols (``xtuner/v1/ops/moe/protocol.py:6-30``),
-backed by the sm_100a C-ABI library.  Same names, argument meaning and error behaviour as the reference's
+backed by the sm_90a C-ABI library.  Same names, argument meaning and error behaviour as the reference's
 ``xtuner.v1.ops.{permute, unpermute, group_gemm}`` and ``xtuner.v1.ops.act_fn.native_swiglu``:
 
 * autograd-aware (``torch.autograd.Function`` over ``torch.library.custom_op`` kernels with fake
@@ -8,7 +8,7 @@ backed by the sm_100a C-ABI library.  Same names, argument meaning and error beh
 * ``tokens_per_expert`` stays a device int64 tensor (no host read);
 * zero-token inputs still join the autograd graph (``ops/moe/cuda/group_gemm.py:34-36``).
 
-There is no fallback: every op raises if the CUDA library is missing or the tensors are not on a B200.
+There is no fallback: every op raises if the CUDA library is missing or the tensors are not on an H100.
 """
 from __future__ import annotations
 

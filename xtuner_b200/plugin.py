@@ -1,4 +1,4 @@
-"""Installs the B200 path into a reference XTuner V1 model without editing the reference tree (INTEGRATION.md §2).
+"""Installs the H100 path into a reference XTuner V1 model without editing the reference tree (INTEGRATION.md §2).
 
 ``convert_model(model)`` walks the reference's modules and, for every ``MoEDecoderLayer``
 (``xtuner/v1/module/decoder_layer/moe_decoder_layer.py:203``):
@@ -76,7 +76,7 @@ def _convert_router(router: nn.Module) -> nn.Module:
         )
         new.e_score_correction_bias = router.e_score_correction_bias  # share the buffer (bias updates keep working)
     else:
-        raise NotImplementedError(f"router {name} has no B200 counterpart (GreedyRouter, NoAuxRouter)")
+        raise NotImplementedError(f"router {name} has no H100 counterpart (GreedyRouter, NoAuxRouter)")
     return new
 
 
@@ -259,7 +259,7 @@ def install_fp8_cast() -> None:
     (``float8/fsdp_utils.py:379-409``) on the local fp32 shard in front of every all-gather — and
     ``tensor_to_per_block_fp8_scales`` (``:75-116``, the per-step scale precompute) when no cross-rank amax reduction is
     involved.  The module functions are looked up by name at call time, so the rebind takes effect for existing tensors.
-    Kernels: bit-exact against reference-made vectors on a B200 (``tests/test_gpu_fp8.py``); this glue: CPU-tested against
+    Kernels: bit-exact against reference-made vectors on an H100 (``tests/test_gpu_fp8.py``); this glue: CPU-tested against
     the reference's functions (``tests/test_plugin_reference_cpu.py``); the two together have not run inside an fp8 training
     step (the reference's fp8 grouped GEMM wheel is absent here)."""
     fu = importlib.import_module("xtuner.v1.float8.fsdp_utils")

@@ -1,6 +1,6 @@
 """Routers with the reference's ``RouterProtocol`` surface (``xtuner/v1/module/router/protocol.py:7-18``):
 ``forward(logits, rollout_routed_experts=None) -> RouterResults`` with the five keys the reference returns
-(including its spelling ``topkens_per_expert``).  One fused sm_100a kernel replaces the reference's
+(including its spelling ``topkens_per_expert``).  One fused sm_90a kernel replaces the reference's
 softmax -> topk -> renorm -> scale -> histc eager chain (``router/greedy.py:64-98``, K6 in SURVEY.md §2.3).
 ``logits`` / ``router_weights`` / ``topk_weights`` stay differentiable (they feed the aux losses and the
 combine, SURVEY.md Appendix B)."""

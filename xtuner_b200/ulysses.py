@@ -11,7 +11,7 @@ while the tensor cores work.  Autograd replays each op on the stream it ran on i
 overlaps the same way without extra code.
 
 The attention kernel itself is the FlashAttention library in this image (``flash_attn`` 2.8, varlen causal GQA) —
-the same call the reference makes (``ops/attn_imp.py:236-267``); a tcgen05 FlashAttention is not built yet
+the same call the reference makes (``ops/attn_imp.py:236-267``); an attention kernel of our own is not built yet
 (DESIGN.md §8).  What is ours here: the exchange (one NVLink hop straight into the ``[S, heads, D]`` layout the
 attention kernel wants — no contiguous/movedim/split/cat copies) and the overlap.
 """
