@@ -395,8 +395,21 @@ def unpermute(input_act: Tensor, row_id_map: Tensor, probs: Tensor | None = None
 
 def group_gemm(x: Tensor, weights: Tensor, split_sizes: Tensor) -> Tensor:
     """``GroupGemmProtocol`` (ops/moe/protocol.py:6-12): ``weights`` is ``[E, dout, din]``,
-    ``split_sizes`` the device int64 ``tokens_per_expert``."""
+    ``split_sizes`` the device int64 ``tokens_per_expert``.
+
+    Shapes are checked on the host before anything is launched (``XtbError``): ``weights`` must be 3-D, ``x`` 2-D with
+    ``x.shape[1] == weights.shape[2]``, and ``split_sizes`` 1-D with ``weights.shape[0]`` entries.  That
+    ``split_sizes`` sums to ``x.shape[0]`` is not checked: the counts live on the device and reading them would
+    synchronise the stream."""
     _require_cuda(x, weights, split_sizes)
+    if weights.dim() != 3:
+        raise _capi.XtbError(f"group_gemm: weights must be [E, dout, din] (got shape {tuple(weights.shape)})")
+    if x.dim() != 2 or x.shape[1] != weights.shape[2]:
+        raise _capi.XtbError(f"group_gemm: x must be [M, {weights.shape[2]}] for weights {tuple(weights.shape)} "
+                             f"(got {tuple(x.shape)})")
+    if split_sizes.dim() != 1 or split_sizes.shape[0] != weights.shape[0]:
+        raise _capi.XtbError(f"group_gemm: split_sizes must be 1-D with {weights.shape[0]} entries, one per expert "
+                             f"(got shape {tuple(split_sizes.shape)})")
     if x.shape[0] == 0:
         return torch.matmul(x, weights[0].T)  # keep x and w in the graph (group_gemm.py:34-36)
     _bf16(x, "x")
