@@ -197,6 +197,27 @@ int xtb_group_gemm_tn(const void* dy, const void* x, const int64_t* tokens_per_e
 int xtb_group_gemm_tn_pair(const void* dy_a, const void* x_a, int N_a, int Kd_a, void* dw_a, const void* dy_b,
                            const void* x_b, int N_b, int Kd_b, void* dw_b, const int64_t* tokens_per_expert,
                            int64_t M_total, int E, xtb_stream_t stream);
+/* ---- f4  lm_head + cross-entropy: loss/ce_loss.py LMHeadLossContext.loss_fn (mode "eager"; "chunk" runs it per chunk)
+ * For T rows of h[T,H] (bf16), head weight w[V,H] (bf16, no bias), labels[T] (int64) and loss_weight[T] (fp32):
+ *   z        = bf16(h . w^T), fp32 accumulation                                   ([T,V] bf16, in z_or_G)
+ *   lsm      = (z - max) - log(sum exp(z - max))  per row, fp32
+ *   row_ce[t]= -lsm[t, labels[t]]  (fp32 [T]);  0 where labels[t] == ignore_index
+ *   *loss    = sum_t row_ce[t] * loss_weight[t]  (fp32 scalar, fixed summation order: identical bits run to run;
+ *              exactly 0 when every row is ignored)
+ * need_grad != 0 additionally (the backward of the above for a loss gradient of 1):
+ *   G        = bf16(exp(lsm) * loss_weight[t] - [v == labels[t]] * loss_weight[t]), written OVER z in z_or_G
+ *              (ignored rows: exactly 0)
+ *   dh[T,H]  = bf16(G . w)      (xtb_group_gemm_nn with one group)
+ *   dW[V,H]  = bf16(G^T . h)    (xtb_group_gemm_tn with one group)
+ * need_grad == 0 leaves z in z_or_G; dh and dW may then be NULL.
+ * A label outside [0, V) that is not ignore_index does not fault: that row's row_ce is NaN (so is the loss, and with
+ * need_grad that row of G).
+ * V % 128 == 0, H % 128 == 0, T < 2^31 (T*V may exceed 2^31: all row offsets are 64-bit).  workspace:
+ * xtb_lm_head_ce_workspace_bytes(T, V) bytes, 16-byte aligned, no initialisation needed. */
+size_t xtb_lm_head_ce_workspace_bytes(int64_t T, int V);
+int xtb_lm_head_ce(const void* h, const void* w, const int64_t* labels, const float* loss_weight, int64_t T, int H, int V,
+                   int64_t ignore_index, int need_grad, void* z_or_G, void* workspace, float* row_ce, float* loss, void* dh,
+                   void* dW, xtb_stream_t stream);
 /* ---- a8  native_swiglu: ops/act_fn.py:7-9 ---------------------------------------------------------
  * out[m, j] = bf16( bf16(silu(h[m, j])) * h[m, I + j] ),  h is [M, 2I] bf16 (gate | up). */
 int xtb_swiglu(const void* h_bf16, void* out_bf16, int64_t M, int I, xtb_stream_t stream);

@@ -112,6 +112,12 @@ SIGNATURES = {
                                        c_int64, c_int64, c_void_p]),
     "xtb_ep_pull_to_sources": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_int64, c_int64, c_int64,
                                        c_void_p]),
+    "xtb_lm_head_ce_workspace_bytes": (c_size_t, [c_int64, c_int]),
+    "xtb_lm_head_ce": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+         c_void_p, c_void_p, c_void_p],
+    ),
     "xtb_swiglu": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "xtb_swiglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
 }

@@ -47,6 +47,11 @@ bool pdl_enabled();  // kernels of the fused MoE path launch with programmatic s
 // points such as cuTensorMapEncodeTiled need one.  Returns XTB_OK or an error status.
 int ensure_context(const void* device_ptr);
 
+// lm_head logits GEMM with the cross-entropy epilogue (group_gemm.cu), driven by xtb_lm_head_ce (lm_head_ce.cu)
+int lm_head_ce_vocab_tiles(int V);
+int lm_head_logits_ce(const void* h, const void* w, const int64_t* tokens_per_expert, int64_t T, int H, int V, void* z,
+                      float2* ce_part, cudaStream_t st);
+
 #define XTB_ENSURE_CTX(ptr)                                   \
   do {                                                        \
     const int _rc = ::xtb::ensure_context(ptr);               \

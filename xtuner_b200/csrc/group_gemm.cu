@@ -64,9 +64,12 @@ struct GemmArgs {
   int n_prob;
   __nv_bfloat16* out_b;
   int m_out_tiles_b, n_tiles_b, ld_out_b;
+  // EPI_CE (lm_head logits, one group): for every row and column tile, (max, sum exp(z - max)) of the stored bf16 logits
+  // z goes to ce_part[row * n_tiles + n_blk]
+  float2* ce_part;
 };
 
-enum GemmEpilogue { EPI_PLAIN = 0, EPI_SWIGLU = 1 };
+enum GemmEpilogue { EPI_PLAIN = 0, EPI_SWIGLU = 1, EPI_CE = 2 };
 
 template <int BLOCK_N, int TA, int TB>
 __device__ __forceinline__ void wgmma_bf16(float (&d)[BLOCK_N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -412,6 +415,42 @@ group_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           }
           emit_box(o_map, o_ptr, o_ld, t.n_blk * BLOCK_N + b * 64, grow, valid, p0, p1);
         }
+        if constexpr (EPI == EPI_CE) {
+          // Statistics of the bf16 logits just stored, from the same rounded values.  Lane (r_lo, qc) holds columns
+          // 8j + 2qc + {0, 1} of row r_lo in acc[4j], acc[4j+1] and of row r_lo + 8 in acc[4j+2], acc[4j+3]; the four
+          // lanes of a quad hold a whole row of the tile.
+          auto bf = [](float x) { return __bfloat162float(__float2bfloat16_rn(x)); };
+          float m0 = __int_as_float(0xff800000), m1 = m0;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            m0 = fmaxf(m0, fmaxf(acc[4 * j], acc[4 * j + 1]));
+            m1 = fmaxf(m1, fmaxf(acc[4 * j + 2], acc[4 * j + 3]));
+          }
+#pragma unroll
+          for (int o = 1; o < 4; o <<= 1) {
+            m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+            m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+          }
+          m0 = bf(m0);  // rounding is monotonic: the max of the rounded row is the rounded max
+          m1 = bf(m1);
+          float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            s0 += expf(bf(acc[4 * j]) - m0);
+            s0 += expf(bf(acc[4 * j + 1]) - m0);
+            s1 += expf(bf(acc[4 * j + 2]) - m1);
+            s1 += expf(bf(acc[4 * j + 3]) - m1);
+          }
+#pragma unroll
+          for (int o = 1; o < 4; o <<= 1) {  // same sum on all four lanes (the two operands of each add commute)
+            s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+          }
+          if (qc == 0) {
+            if (r_lo < valid) args.ce_part[(size_t)(grow + r_lo) * args.n_tiles + t.n_blk] = make_float2(m0, s0);
+            if (r_lo + 8 < valid) args.ce_part[(size_t)(grow + r_lo + 8) * args.n_tiles + t.n_blk] = make_float2(m1, s1);
+          }
+        }
       }
     }
     if constexpr (STORE) {
@@ -505,6 +544,26 @@ static int check_common(const void* a, const void* b, const int64_t* tpe, void* 
   return XTB_OK;
 }
 
+// NT output tile width: 256 columns where N allows, else 128
+static int nt_block_n(int N) { return (N % 256 == 0) ? 256 : 128; }
+
+// The NT product of xtb_group_gemm_nt; `a` arrives with tokens_per_expert, out and the epilogue's own fields set.
+template <int EPI>
+static int launch_nt(const void* x, const void* w, int64_t M_total, int N, int Kd, int E, GemmArgs a, cudaStream_t st) {
+  const int BN = nt_block_n(N);
+  CUtensorMap ta, tb;
+  int rc;
+  if ((rc = make_tmap(&ta, x, (uint64_t)M_total, (uint64_t)Kd, BLOCK_M, BLOCK_K))) return rc;
+  if ((rc = make_tmap(&tb, w, (uint64_t)E * N, (uint64_t)Kd, BN, BLOCK_K))) return rc;
+  a.E = E;
+  a.n_tiles = N / BN;
+  a.k_red = Kd;
+  a.ld_out = N;
+  a.w_rows = N;
+  if (BN == 256) return launch_gemm<MODE_NT, 256, EPI>(ta, tb, a, (uint64_t)M_total, st);
+  return launch_gemm<MODE_NT, 128, EPI>(ta, tb, a, (uint64_t)M_total, st);
+}
+
 }  // namespace xtb
 
 using namespace xtb;
@@ -525,20 +584,24 @@ extern "C" int xtb_group_gemm_nt(const void* x, const void* w, const int64_t* to
   int rc = check_common(x, w, tokens_per_expert, out, M_total, N, Kd, E, "xtb_group_gemm_nt");
   if (rc) return rc;
   if (M_total == 0) return XTB_OK;
-  const int BN = (N % 256 == 0) ? 256 : 128;
-  CUtensorMap ta, tb;
-  if ((rc = make_tmap(&ta, x, (uint64_t)M_total, (uint64_t)Kd, BLOCK_M, BLOCK_K))) return rc;
-  if ((rc = make_tmap(&tb, w, (uint64_t)E * N, (uint64_t)Kd, BN, BLOCK_K))) return rc;
   GemmArgs a{};
   a.tokens_per_expert = tokens_per_expert;
   a.out = static_cast<__nv_bfloat16*>(out);
-  a.E = E;
-  a.n_tiles = N / BN;
-  a.k_red = Kd;
-  a.ld_out = N;
-  a.w_rows = N;
-  if (BN == 256) return launch_gemm<MODE_NT, 256>(ta, tb, a, (uint64_t)M_total, as_stream(stream));
-  return launch_gemm<MODE_NT, 128>(ta, tb, a, (uint64_t)M_total, as_stream(stream));
+  return launch_nt<EPI_PLAIN>(x, w, M_total, N, Kd, E, a, as_stream(stream));
+}
+
+// The lm_head logits of xtb_lm_head_ce (csrc/lm_head_ce.cu): z[T, V] = bf16(h[T, H] . w[V, H]^T), the NT product with one
+// group (tokens_per_expert = {T} on the device) and the EPI_CE epilogue.  ce_part holds lm_head_ce_vocab_tiles(V) entries
+// per row.
+int xtb::lm_head_ce_vocab_tiles(int V) { return V / nt_block_n(V); }
+
+int xtb::lm_head_logits_ce(const void* h, const void* w, const int64_t* tokens_per_expert, int64_t T, int H, int V,
+                           void* z, float2* ce_part, cudaStream_t st) {
+  GemmArgs a{};
+  a.tokens_per_expert = tokens_per_expert;
+  a.out = static_cast<__nv_bfloat16*>(z);
+  a.ce_part = ce_part;
+  return launch_nt<EPI_CE>(h, w, T, V, H, 1, a, st);
 }
 
 extern "C" int xtb_group_gemm_nt_swiglu(const void* x, const void* w13, const int64_t* tokens_per_expert,

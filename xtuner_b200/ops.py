@@ -20,7 +20,7 @@ from torch import Tensor
 from . import _capi
 from ._capi import check, current_stream, ptr
 
-__all__ = ["permute", "unpermute", "group_gemm", "swiglu", "gate_logits", "permute_workspace"]
+__all__ = ["permute", "unpermute", "group_gemm", "swiglu", "gate_logits", "permute_workspace", "lm_head_cross_entropy"]
 
 
 def _require_cuda(*tensors: Tensor) -> None:
@@ -438,6 +438,88 @@ def gate_logits(hidden_states: Tensor, weight: Tensor, bias: Tensor | None = Non
     w = weight if weight.dtype == torch.float32 else weight.float()
     b = None if bias is None else bias.float().contiguous()
     return _GateLogits.apply(x, w.contiguous(), b)
+
+
+# ======================================================================================================
+# lm_head + cross-entropy (f4): what LMHeadLossContext computes in modes "eager" and "chunk"
+# ======================================================================================================
+
+
+def _lm_head_ce_call(h, w, labels, loss_weight, ignore_index, need_grad, z, row_ce, loss, dh, dw) -> None:
+    lib = _capi.ensure_init()
+    T, H = h.shape
+    V = w.shape[0]
+    ws = _scratch("lm_head_ce", int(lib.xtb_lm_head_ce_workspace_bytes(T, V)), h.device)
+    check(
+        lib.xtb_lm_head_ce(
+            ptr(h), ptr(w), ptr(labels), ptr(loss_weight), T, H, V, ignore_index, int(need_grad), ptr(z), ptr(ws),
+            ptr(row_ce), ptr(loss), ptr(dh), ptr(dw), current_stream(),
+        ),
+        "xtb_lm_head_ce",
+    )
+
+
+class _LMHeadCrossEntropy(torch.autograd.Function):
+    """``ChunkLoss`` (loss/chunk_loss.py) over ``xtb_lm_head_ce``: the gradients are computed in the forward, one row chunk
+    at a time (one chunk = eager semantics); chunk losses are added in fp32 and each later chunk's ``dW`` is added into
+    the first in bf16, in chunk order.  Backward scales both by ``grad_output`` on the device."""
+
+    @staticmethod
+    def forward(ctx, h: Tensor, w: Tensor, labels: Tensor, loss_weight: Tensor, ignore_index: int,
+                chunk_size: Optional[int], need_grad: bool):
+        T = h.shape[0]
+        step = max(T, 1) if chunk_size is None else chunk_size
+        z = torch.empty((min(step, T), w.shape[0]), dtype=torch.bfloat16, device=h.device)  # z, then G, of one chunk
+        row_ce = torch.empty((T,), dtype=torch.float32, device=h.device)
+        dh = torch.empty_like(h) if need_grad else None
+        loss = dw = dw_chunk = None
+        for s in range(0, max(T, 1), step):
+            n = min(step, T - s)
+            loss_c = torch.empty((), dtype=torch.float32, device=h.device)
+            dw_c = None
+            if need_grad:  # the first chunk writes dW itself, later ones a scratch copy that is added into it
+                dw_chunk = torch.empty_like(w) if dw is not None and dw_chunk is None else dw_chunk
+                dw_c = torch.empty_like(w) if dw is None else dw_chunk
+            _lm_head_ce_call(h[s:s + n], w, labels[s:s + n], loss_weight[s:s + n], ignore_index, need_grad, z[:n],
+                             row_ce[s:s + n], loss_c, None if dh is None else dh[s:s + n], dw_c)
+            loss = loss_c if loss is None else loss.add_(loss_c)
+            if need_grad:
+                dw = dw_c if dw is None else dw.add_(dw_c)
+        if need_grad:
+            ctx.save_for_backward(dh, dw)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        dh, dw = ctx.saved_tensors
+        # unconditional: x1 is exact, so this equals ChunkLoss's `if grad_output != 1` without reading it on the host
+        return (dh * grad_output if ctx.needs_input_grad[0] else None,
+                dw * grad_output if ctx.needs_input_grad[1] else None, None, None, None, None, None)
+
+
+def lm_head_cross_entropy(hidden: Tensor, weight: Tensor, labels: Tensor, loss_weight: Tensor, ignore_index: int = -100,
+                          chunk_size: int | None = None) -> Tensor:
+    """``sum_t CE(hidden[t] . weight^T, labels[t]) * loss_weight[t]`` as ``LMHeadLossContext`` computes it
+    (loss/ce_loss.py ``loss_fn``): bf16 logits, fp32 log-softmax, rows with ``labels == ignore_index`` contribute 0.
+    ``chunk_size=None`` is mode "eager"; an integer runs mode "chunk" (``ChunkLoss``) over rows of that many.
+    ``hidden`` is ``[..., H]`` bf16, ``weight`` ``[V, H]`` bf16 with ``V % 128 == 0`` and ``H % 128 == 0``, ``labels`` and
+    ``loss_weight`` hold one entry per row of ``hidden``.  The logits are never returned: one bf16 ``[rows, V]`` buffer per
+    chunk holds them and then their gradient.  Gradients are computed in the forward when grad mode is on and ``hidden``
+    or ``weight`` requires grad.  A label outside ``[0, V)`` that is not ``ignore_index`` makes the loss NaN."""
+    _require_cuda(hidden, weight, labels, loss_weight)
+    _bf16(hidden, "hidden")
+    _bf16(weight, "weight")
+    if weight.dim() != 2 or hidden.shape[-1] != weight.shape[1]:
+        raise _capi.XtbError(f"lm_head_cross_entropy: weight must be [V, {hidden.shape[-1]}] (got {tuple(weight.shape)})")
+    h = hidden.reshape(-1, hidden.shape[-1]).contiguous()
+    lab = labels.reshape(-1).to(torch.int64).contiguous()
+    lw = loss_weight.reshape(-1).to(torch.float32).contiguous()
+    if lab.numel() != h.shape[0] or lw.numel() != h.shape[0]:
+        raise _capi.XtbError(f"lm_head_cross_entropy: {h.shape[0]} rows but {lab.numel()} labels and {lw.numel()} weights")
+    if chunk_size is not None and chunk_size <= 0:
+        raise ValueError(f"lm_head_cross_entropy: chunk_size must be positive (got {chunk_size})")
+    need_grad = torch.is_grad_enabled() and (hidden.requires_grad or weight.requires_grad)
+    return _LMHeadCrossEntropy.apply(h, weight.contiguous(), lab, lw, int(ignore_index), chunk_size, need_grad)
 
 
 # ======================================================================================================

@@ -15,7 +15,8 @@ experts -> combine -> ``* hidden_factor + residual``, ``moe_decoder_layer.py:668
 autograd node (:func:`xtuner_b200.fused.fused_moe_block`), the form ``bench.py`` measures; the per-op classes above stay
 installed for the paths the fused node does not cover (micro-batched forward, rollout-routed experts).
 
-Everything else of the model (attention, norms, lm_head, FSDP wrapping, checkpoint keys) is untouched; parameters keep
+Everything else of the model (attention, norms, lm_head, FSDP wrapping, checkpoint keys) is untouched;
+``install_lm_head_loss()`` separately moves the lm_head cross-entropy onto this package's kernels; parameters keep
 their names, so state dicts and DCP checkpoints stay compatible.  ``restore_model`` undoes the conversion.
 """
 from __future__ import annotations
@@ -235,6 +236,68 @@ def uninstall_ulysses() -> None:
     if hasattr(mha, _SAVED):
         mha.ulysses_all_to_all = getattr(mha, _SAVED)
         delattr(mha, _SAVED)
+
+
+# ======================================================================================================
+# lm_head + cross-entropy (f4)
+# ======================================================================================================
+
+
+def _lm_head_eligible(ctx, cls, hidden_states, head_weight, head_bias) -> bool:
+    """what ``ops.lm_head_cross_entropy`` computes: the plain context (``MTPLossContext`` subclasses it with its own
+    ``loss_fn``), no bias, bf16 CUDA hidden states and weight (``fp32_lm_head`` gives fp32), widths multiples of 128"""
+    kw = ctx.loss_kwargs
+    return (type(ctx) is cls and head_bias is None and kw is not None and kw.loss_weight is not None
+            and all(type(t) in (torch.Tensor, nn.Parameter) and _on_device(t) and t.dtype == torch.bfloat16
+                    for t in (hidden_states, head_weight))
+            and head_weight.dim() == 2 and head_weight.shape[0] % 128 == 0 and head_weight.shape[1] % 128 == 0)
+
+
+def _lm_head_loss(ctx, hidden_states, head_weight, loss_kwargs, chunk_size):
+    loss = ops.lm_head_cross_entropy(hidden_states, head_weight, loss_kwargs.shifted_labels, loss_kwargs.loss_weight,
+                                     ctx.loss_cfg.ignore_idx, chunk_size)
+    return loss, (None, {})
+
+
+def install_lm_head_loss() -> None:
+    """Rebinds ``LMHeadLossContext.eager_mode`` and ``.chunk_mode`` (``xtuner/v1/loss/ce_loss.py``) so that modes
+    ``"eager"`` and ``"chunk"`` run :func:`ops.lm_head_cross_entropy`: the logits GEMM with the cross-entropy epilogue, the
+    loss and both gradients on this package's kernels, with the reference's roundings.  Calls it does not cover go to the
+    original methods: subclasses such as ``MTPLossContext``, mode ``"liger"``, a head bias, fp32 or non-CUDA tensors,
+    ``V`` or ``H`` not a multiple of 128, and chunk mode over a batch of more than one sequence (``ChunkLoss`` splits
+    along the sequence dimension of each).
+
+    Opt-in because it changes one output: like chunk mode, the served calls return ``(loss, (None, {}))``, so in eager
+    mode the fp32 logits that the reference returns, and that end up in ``MoEModelOutputs.logits``, are not produced."""
+    ce = importlib.import_module("xtuner.v1.loss.ce_loss")
+    cls = ce.LMHeadLossContext
+    if _SAVED in vars(cls):
+        return
+    orig_eager, orig_chunk = vars(cls)["eager_mode"], vars(cls)["chunk_mode"]
+
+    def eager_mode(self, hidden_states, head_weight, head_bias, loss_kwargs):
+        if self.loss_cfg.mode == "eager" and _lm_head_eligible(self, cls, hidden_states, head_weight, head_bias):
+            return _lm_head_loss(self, hidden_states, head_weight, loss_kwargs, None)
+        return orig_eager(self, hidden_states, head_weight, head_bias, loss_kwargs)
+
+    def chunk_mode(self, hidden_states, head_weight, head_bias, loss_kwargs):
+        if (self.loss_cfg.mode == "chunk" and self.loss_cfg.chunk_size is not None
+                and (hidden_states.dim() == 2 or hidden_states.shape[0] == 1)
+                and _lm_head_eligible(self, cls, hidden_states, head_weight, head_bias)):
+            return _lm_head_loss(self, hidden_states, head_weight, loss_kwargs, self.loss_cfg.chunk_size)
+        return orig_chunk(self, hidden_states, head_weight, head_bias, loss_kwargs)
+
+    eager_mode.__wrapped__, chunk_mode.__wrapped__ = orig_eager, orig_chunk
+    setattr(cls, _SAVED, (orig_eager, orig_chunk))
+    cls.eager_mode, cls.chunk_mode = eager_mode, chunk_mode
+
+
+def uninstall_lm_head_loss() -> None:
+    ce = importlib.import_module("xtuner.v1.loss.ce_loss")
+    cls = ce.LMHeadLossContext
+    if _SAVED in vars(cls):
+        cls.eager_mode, cls.chunk_mode = vars(cls)[_SAVED]
+        delattr(cls, _SAVED)
 
 
 # ======================================================================================================
