@@ -518,7 +518,7 @@ extern "C" int xtb_rmsnorm_gate(const void* h_bf16, const float* norm_w_f32, con
   XTB_CHECK_ARG(H == 256 || H == 512 || H == 1024 || H == 2048,
                 "xtb_rmsnorm_gate: unsupported H=%d (256, 512, 1024, 2048: the row lives in registers)", H);
   if (!gate_w_f32) {
-    // norm only: column-owned streaming kernel, 4 tokens per 256-thread block, any H % 8 == 0
+    // norm only: column-owned streaming kernel, 4 tokens per 256-thread block (one 8-column vector per thread)
     XTB_CUDA(launch_pdl(rmsnorm_cols_kernel<4>, dim3((T + 3) / 4), dim3(256), 0, st, hp, norm_w_f32, xp, rstd_out, T, H, eps));
     XTB_LAUNCH_OK();
     return XTB_OK;

@@ -536,11 +536,12 @@ extern "C" int xtb_moe_permute_index(const int32_t* ids, int T, int K, int E, in
                       stream, false);
 }
 
-extern "C" int xtb_moe_combine(const void* y_bf16, const int32_t* row_id_map, const float* probs,
-                               const void* residual_bf16, float hidden_factor, int T, int K, int H, void* out_bf16,
-                               xtb_stream_t stream) {
-  XTB_CHECK_ARG(y_bf16 && row_id_map && out_bf16, "xtb_moe_unpermute: null pointer");
-  XTB_CHECK_ARG(T >= 0 && K > 0 && H > 0 && H % 8 == 0, "xtb_moe_unpermute: bad T=%d K=%d H=%d (H%%8==0)", T, K, H);
+// xtb_moe_combine and xtb_moe_unpermute; `entry` names the one that was called in the refusal messages
+static int combine_impl(const char* entry, const void* y_bf16, const int32_t* row_id_map, const float* probs,
+                        const void* residual_bf16, float hidden_factor, int T, int K, int H, void* out_bf16,
+                        xtb_stream_t stream) {
+  XTB_CHECK_ARG(y_bf16 && row_id_map && out_bf16, "%s: null pointer", entry);
+  XTB_CHECK_ARG(T >= 0 && K > 0 && H > 0 && H % 8 == 0, "%s: bad T=%d K=%d H=%d (H%%8==0)", entry, T, K, H);
   XTB_ENSURE_CTX(y_bf16);
   if (T == 0) return XTB_OK;
   cudaStream_t st = as_stream(stream);
@@ -563,9 +564,16 @@ extern "C" int xtb_moe_combine(const void* y_bf16, const int32_t* row_id_map, co
   return XTB_OK;
 }
 
+extern "C" int xtb_moe_combine(const void* y_bf16, const int32_t* row_id_map, const float* probs,
+                               const void* residual_bf16, float hidden_factor, int T, int K, int H, void* out_bf16,
+                               xtb_stream_t stream) {
+  return combine_impl("xtb_moe_combine", y_bf16, row_id_map, probs, residual_bf16, hidden_factor, T, K, H, out_bf16,
+                      stream);
+}
+
 extern "C" int xtb_moe_unpermute(const void* y_bf16, const int32_t* row_id_map, const float* probs, int T, int K,
                                  int H, void* out_bf16, xtb_stream_t stream) {
-  return xtb_moe_combine(y_bf16, row_id_map, probs, nullptr, 1.0f, T, K, H, out_bf16, stream);
+  return combine_impl("xtb_moe_unpermute", y_bf16, row_id_map, probs, nullptr, 1.0f, T, K, H, out_bf16, stream);
 }
 
 extern "C" int xtb_moe_unpermute_bwd(const void* grad_out_bf16, const void* y_fwd_bf16, const int32_t* row_id_map,
