@@ -120,11 +120,15 @@ int xtb_router_noaux(const float* logits, const float* e_score_correction_bias, 
                      xtb_stream_t stream);
 
 /* backward of a2' (what autograd does to noaux_router.py:80-134; closed form in oracle/moe_oracle.py
- * noaux_router_bwd).  Inputs are the forward's inputs and outputs; has_group_mask = (n_group != topk_group): the
- * kept-group mask is recovered as router_weights != 0 (masked_fill(…, 0.0), :113).  Either grad may be NULL. */
+ * noaux_router_bwd).  Inputs are the forward's inputs and outputs, and its group geometry as
+ * group_spec = XTB_NOAUX_GROUP_SPEC(n_group, topk_group): 0 when n_group == topk_group (no group mask), otherwise
+ * n_group | topk_group << 8.  The kept-group mask is recomputed from logits and bias: a kept expert's router weight may
+ * be exactly 0, so router_weights != 0 does not identify it.  Either grad may be NULL. */
+#define XTB_NOAUX_GROUP_SPEC(n_group, topk_group) \
+  ((n_group) == (topk_group) ? 0 : ((n_group) | ((topk_group) << 8)))
 int xtb_router_noaux_bwd(const float* logits, const float* e_score_correction_bias, const float* router_weights,
                          const float* topk_weights, const int64_t* topk_ids, const float* grad_topk_weights,
-                         const float* grad_router_weights, int T, int E, int K, int has_group_mask,
+                         const float* grad_router_weights, int T, int E, int K, int group_spec,
                          int norm_topk_prob, float scaling, float* grad_logits, xtb_stream_t stream);
 
 /* ---- a4  permute: ops/moe/protocol.py:15-23, ops/moe/cuda/permute_unpermute.py:92-143,205-219 -------

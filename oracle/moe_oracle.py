@@ -113,6 +113,20 @@ def noaux_router(
     }
 
 
+def noaux_kept_experts(scores_for_choice: torch.Tensor, n_group: int, topk_group: int) -> torch.Tensor:
+    """bool [T, E]: the experts whose group ``noaux_router`` keeps (noaux_router.py:91-113), all True when
+    ``n_group == topk_group``.  Group score = largest + second largest choice score of the group; groups tied on the
+    score are taken lowest index first (what the CUDA kernels do; ``topk(sorted=False)`` leaves the order open)."""
+    n_tok, n_experts = scores_for_choice.shape
+    if n_group == topk_group:
+        return torch.ones_like(scores_for_choice, dtype=torch.bool)
+    group_scores = scores_for_choice.view(n_tok, n_group, -1).topk(2, dim=-1)[0].sum(dim=-1)
+    order = torch.sort(group_scores, dim=-1, descending=True, stable=True)[1]
+    group_mask = torch.zeros_like(group_scores, dtype=torch.bool)
+    group_mask.scatter_(1, order[:, :topk_group], True)
+    return group_mask.repeat_interleave(n_experts // n_group, dim=1)
+
+
 def noaux_router_bwd(
     logits: torch.Tensor,
     e_score_correction_bias: torch.Tensor,
@@ -124,14 +138,28 @@ def noaux_router_bwd(
     has_group_mask: bool,
     router_scaling_factor: float,
     norm_topk_prob: bool = True,
+    n_group: Optional[int] = None,
+    topk_group: Optional[int] = None,
 ) -> torch.Tensor:
     """Closed form of what autograd does to ``noaux_router`` (noaux_router.py:80,85,113,125-134): the restatement the
-    CUDA backward follows.  The group mask is recovered from the forward output (``router_weights != 0``; the masked
-    choice scores are exactly 0.0 after ``masked_fill``, :113) instead of re-running the group selection."""
+    CUDA backward follows.  With ``n_group`` and ``topk_group`` the group mask is recomputed from logits and bias
+    (:func:`noaux_kept_experts`), as the CUDA backward does.  Without them it is read back as ``router_weights != 0``
+    (masked choice scores are exactly 0.0 after ``masked_fill``, :113).  That read-back cannot tell a masked expert from
+    a kept one whose choice score is exactly 0 (router weight 0, gradient (g - dot) / S), so it raises on such rows
+    instead of dropping that gradient."""
     s = torch.sigmoid(logits)
     ds = torch.zeros_like(s)
     if grad_router_weights is not None:
-        mask = (router_weights != 0) if has_group_mask else torch.ones_like(s, dtype=torch.bool)
+        ch = s + e_score_correction_bias.unsqueeze(0)
+        if not has_group_mask:
+            mask = torch.ones_like(s, dtype=torch.bool)
+        elif n_group is not None and topk_group is not None:
+            mask = noaux_kept_experts(ch, n_group, topk_group)
+        else:
+            mask = router_weights != 0
+            if bool(((ch == 0) & ~mask).any()):
+                raise ValueError("noaux_router_bwd: a choice score is exactly 0, so router_weights != 0 does not give "
+                                 "the group mask; pass n_group and topk_group")
         c = torch.where(mask, s + e_score_correction_bias.unsqueeze(0), torch.zeros_like(s))
         S = c.sum(dim=-1, keepdim=True)
         dot = (grad_router_weights * router_weights).sum(dim=-1, keepdim=True)

@@ -102,12 +102,13 @@ class EmulatedLib:
         _view(tpe, torch.float32, E).copy_(r["topkens_per_expert"])
         return 0
 
-    def xtb_router_noaux_bwd(self, logits, bias, rw, tw, ids, g_tw, g_rw, T, E, K, has_mask, norm, scaling, gl, stream):
+    def xtb_router_noaux_bwd(self, logits, bias, rw, tw, ids, g_tw, g_rw, T, E, K, group_spec, norm, scaling, gl, stream):
         self.calls.append("xtb_router_noaux_bwd")
         out = O.noaux_router_bwd(
             _view(logits, torch.float32, T, E), _view(bias, torch.float32, E), _view(rw, torch.float32, T, E),
             _view(tw, torch.float32, T, K), _view(ids, torch.int64, T, K), _view(g_tw, torch.float32, T, K),
-            _view(g_rw, torch.float32, T, E), bool(has_mask), scaling, bool(norm))
+            _view(g_rw, torch.float32, T, E), group_spec != 0, scaling, bool(norm), n_group=group_spec & 0xFF,
+            topk_group=group_spec >> 8)
         _view(gl, torch.float32, T, E).copy_(out)
         return 0
 

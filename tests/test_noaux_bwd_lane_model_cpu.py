@@ -1,7 +1,9 @@
 """Lane-level model of ``router_noaux_bwd_kernel<LPT, VPL>`` (csrc/route.cu): LPT lanes per token, each holding VPL
-consecutive experts, xor-shuffle reductions for the row sums, the group mask read back from ``router_weights != 0``, the
-top-k gradient scattered by id.  Restates the kernel's per-lane arithmetic and checks it against the reference-made
-gradient fixture — the kernel itself is covered on the GPU by tests/test_gpu_router.py (noaux backward vs the same fixture)."""
+consecutive experts, xor-shuffle reductions for the row sums, the group mask recomputed from the choice scores
+(``noaux_kept_experts``: per-lane top-2, xor merges across the lanes of a group, topk_group butterfly arg-max rounds),
+the top-k gradient scattered by id.  Restates the kernel's per-lane arithmetic and checks it against the reference-made
+gradient fixture and against the forward's group choice — the kernel itself is covered on the GPU by
+tests/test_gpu_router.py and tests/test_gpu_router_edges.py."""
 import numpy as np
 import pytest
 import torch
@@ -9,7 +11,61 @@ import torch
 from tests.conftest import load_golden
 
 
-def lane_model(logits, bias, rw, tw, ids, g_tw, g_rw, has_mask, norm_topk, scaling, LPT, VPL):
+def top2_insert(a, b, v):
+    if v > a:
+        return v, a
+    if v > b:
+        return a, v
+    return a, b
+
+
+def kept_lane_model(ch, n_group, topk_group, LPT, VPL):
+    """``noaux_kept_experts<LPT, VPL>`` for one token: ``ch`` float32 [E] -> bool [E]."""
+    E = ch.shape[0]
+    f32 = np.float32
+    gs = E // n_group
+    ninf = f32(-np.inf)
+    gv = np.full((LPT, VPL), ninf, f32)
+    cand = np.zeros((LPT, VPL), bool)
+    a = np.full(LPT, ninf, f32)
+    b = np.full(LPT, ninf, f32)
+    for sub in range(LPT):
+        for j in range(VPL):
+            a[sub], b[sub] = top2_insert(a[sub], b[sub], ch[sub * VPL + j])
+            if gs <= VPL and (j + 1) % gs == 0:
+                gv[sub, j] = f32(a[sub] + b[sub])
+                cand[sub, j] = True
+                a[sub] = b[sub] = ninf
+    if gs > VPL:
+        o = 1
+        while o < gs // VPL:
+            oa, ob = a[np.arange(LPT) ^ o], b[np.arange(LPT) ^ o]
+            a, b = np.maximum(a, oa), np.maximum(np.minimum(a, oa), np.maximum(b, ob))
+            o *= 2
+        for sub in range(LPT):
+            gv[sub, VPL - 1] = f32(a[sub] + b[sub])
+            cand[sub, VPL - 1] = (sub * VPL) % gs == 0
+    kept = set()
+    for _ in range(topk_group):
+        bv = np.full(LPT, ninf, f32)
+        bi = np.full(LPT, 2**31 - 1, np.int64)
+        for sub in range(LPT):
+            for j in range(VPL):
+                gi = (sub * VPL + j) // gs
+                if cand[sub, j] and gi not in kept and (gv[sub, j] > bv[sub] or (gv[sub, j] == bv[sub] and gi < bi[sub])):
+                    bv[sub], bi[sub] = gv[sub, j], gi
+        o = LPT // 2
+        while o > 0:
+            ov, oi = bv[np.arange(LPT) ^ o], bi[np.arange(LPT) ^ o]
+            take = (ov > bv) | ((ov == bv) & (oi < bi))
+            bv, bi = np.where(take, ov, bv), np.where(take, oi, bi)
+            o //= 2
+        assert (bi == bi[0]).all()  # every lane of the token agrees
+        kept.add(int(bi[0]))
+    return np.array([(e // gs) in kept for e in range(E)])
+
+
+def lane_model(logits, bias, rw, tw, ids, g_tw, g_rw, n_group, topk_group, norm_topk, scaling, LPT, VPL):
     T, E = logits.shape
     K = ids.shape[1]
     out = np.zeros((T, E), np.float32)
@@ -24,6 +80,11 @@ def lane_model(logits, bias, rw, tw, ids, g_tw, g_rw, has_mask, norm_topk, scali
                 sg[j] = f32(1) / (f32(1) + np.exp(-x, dtype=f32))
             lanes.append(dict(e0=e0, sg=sg, ds=np.zeros(VPL, f32)))
         if g_rw is not None:
+            if n_group != topk_group:
+                ch = np.concatenate([ln["sg"] for ln in lanes]) + bias.astype(f32)
+                kept = kept_lane_model(ch.astype(f32), n_group, topk_group, LPT, VPL)
+            else:
+                kept = np.ones(E, bool)
             S = np.zeros(LPT, f32)
             dot = np.zeros(LPT, f32)
             for sub, ln in enumerate(lanes):
@@ -33,7 +94,7 @@ def lane_model(logits, bias, rw, tw, ids, g_tw, g_rw, has_mask, norm_topk, scali
                     e = ln["e0"] + j
                     r = rw[tok, e] if e < E else f32(0)
                     ln["g"][j] = g_rw[tok, e] if e < E else f32(0)
-                    ln["keep"][j] = (e < E) and (not has_mask or r != 0)
+                    ln["keep"][j] = (e < E) and kept[e]
                     if ln["keep"][j]:
                         S[sub] += ln["sg"][j] + bias[e]
                     dot[sub] = f32(ln["g"][j] * r + dot[sub])
@@ -85,7 +146,7 @@ def test_noaux_bwd_lane_model(tag):
     a = lambda k: g[k][:n].numpy()
     LPT, VPL = dispatch(g["logits"].shape[1])
     common = (a("logits"), g["e_score_correction_bias"].numpy(), a("router_weights"), a("topk_weights"), a("topk_ids"))
-    tail = (g["n_group"] != g["topk_group"], g["norm_topk_prob"], g["router_scaling_factor"], LPT, VPL)
+    tail = (g["n_group"], g["topk_group"], g["norm_topk_prob"], g["router_scaling_factor"], LPT, VPL)
     with np.errstate(over="ignore"):
         both = lane_model(*common, a("grad_topk_weights"), a("grad_router_weights"), *tail)
         only_tw = lane_model(*common, a("grad_topk_weights"), None, *tail)
@@ -93,3 +154,70 @@ def test_noaux_bwd_lane_model(tag):
     np.testing.assert_allclose(both, a("grad_logits"), rtol=2e-5, atol=2e-6)
     np.testing.assert_allclose(only_tw, a("grad_logits_from_topk"), rtol=2e-5, atol=2e-6)
     np.testing.assert_allclose(only_rw, a("grad_logits_from_router_weights"), rtol=2e-5, atol=2e-6)
+
+
+@pytest.mark.parametrize("E,n_group,topk_group", [(32, 4, 2), (32, 16, 3), (64, 8, 3), (128, 32, 5), (256, 8, 4),
+                                                  (256, 2, 1), (512, 16, 4), (512, 4, 3), (512, 32, 7)])
+def test_kept_experts_lane_model_equals_the_forward_choice(E, n_group, topk_group):
+    """The backward's recomputed group mask, under the backward's lane mapping (groups inside one lane and groups
+    spanning 2 to 32 lanes), equals the group choice of the forward: the oracle's mask, and the experts the forward's
+    router_weights leave non-zero.  Rows include tied group scores (lowest group index first)."""
+    from oracle import moe_oracle as O
+
+    LPT, VPL = dispatch(E)
+    g = torch.Generator().manual_seed(E + n_group)
+    T = 6
+    logits = torch.randn(T, E, generator=g)
+    logits[0] = 0.0  # every group ties
+    logits[1, : E // 2] = logits[1, E // 2 :]  # the two halves' groups tie pairwise
+    bias = torch.randn(E, generator=g) * 0.1
+    ch = torch.sigmoid(logits) + bias
+    ch[0] = 0.25
+    want = O.noaux_kept_experts(ch, n_group, topk_group)
+    for t in range(T):
+        got = kept_lane_model(ch[t].numpy(), n_group, topk_group, LPT, VPL)
+        assert (got == want[t].numpy()).all(), t
+    assert (want.view(T, n_group, -1).all(-1).sum(-1) == topk_group).all()
+    assert torch.equal(want[0].view(n_group, -1).all(-1).nonzero().flatten(), torch.arange(topk_group))
+    fwd = O.noaux_router(logits[2:], bias, min(8, E // n_group * topk_group), n_group, topk_group, 1.0)
+    assert torch.equal(fwd["router_weights"] != 0, want[2:])
+
+
+def test_zero_score_kept_expert_keeps_its_router_weight_gradient():
+    """A kept expert whose choice score is exactly 0 (logit 0 gives sigmoid 0.5, bias -0.5): its router weight is 0,
+    and autograd still gives it (g - dot) / S sigma'.  A mask read back from router_weights != 0 drops that gradient;
+    the recomputed mask keeps it."""
+    from oracle import moe_oracle as O
+
+    E, NG, TG, K = 64, 8, 4, 4
+    g = torch.Generator().manual_seed(3)
+    logits = torch.randn(2, E, generator=g)
+    bias = torch.zeros(E)
+    logits[:, 0:8] = 4.0  # group 0 is kept
+    logits[:, 3] = 0.0
+    bias[3] = -0.5
+    lg = logits.clone().requires_grad_(True)
+    r = O.noaux_router(lg, bias, K, NG, TG, 1.0)
+    assert float(r["router_weights"][0, 3]) == 0.0 and bool((r["router_weights"][:, 0:8].sum(-1) > 0).all())
+    g_rw = torch.randn(2, E, generator=g)
+    (want,) = torch.autograd.grad(r["router_weights"], lg, g_rw)
+    assert float(want[0, 3]) != 0.0
+    rw, tw, ids = (r[k].detach() for k in ("router_weights", "topk_weights", "topk_ids"))
+    got = O.noaux_router_bwd(logits, bias, rw, tw, ids, None, g_rw, True, 1.0, n_group=NG, topk_group=TG)
+    torch.testing.assert_close(got, want, rtol=2e-5, atol=2e-6)
+    LPT, VPL = dispatch(E)
+    lane = lane_model(logits.numpy(), bias.numpy(), rw.numpy(), tw.numpy(), ids.numpy(), None, g_rw.numpy(), NG, TG,
+                      True, 1.0, LPT, VPL)
+    np.testing.assert_allclose(lane, want.numpy(), rtol=2e-5, atol=2e-6)
+
+    # without the geometry the oracle would have to read the mask back from router_weights != 0: it refuses this row
+    with pytest.raises(ValueError, match="exactly 0"):
+        O.noaux_router_bwd(logits, bias, rw, tw, ids, None, g_rw, True, 1.0)
+    # the closed form the backward used before: the group mask read back from router_weights != 0
+    s = torch.sigmoid(logits)
+    mask = rw != 0
+    c = torch.where(mask, s + bias, torch.zeros_like(s))
+    dot = (g_rw * rw).sum(-1, keepdim=True)
+    old = torch.where(mask, (g_rw - dot) / c.sum(-1, keepdim=True), torch.zeros_like(s)) * s * (1 - s)
+    assert float(old[0, 3]) == 0.0
+    assert not torch.allclose(old, want, rtol=2e-5, atol=2e-6)

@@ -219,8 +219,8 @@ __device__ __forceinline__ void route_token_e8(const float* __restrict__ lg, int
         be = j;
       }
     }
-    if (be < 0 || be >= E) {  // NaN rows: stay in range (as the router kernel does)
-      be = k;
+    if (be < 0 || be >= E) {  // NaN rows: the lowest index not selected yet, as the router kernel does (at most k < E)
+      be = __ffs(~taken) - 1;
       bv = 0.f;
     }
     taken |= 1u << be;
@@ -373,7 +373,7 @@ extern "C" int xtb_gate_route_dispatch(const void* x_bf16, const float* w_f32, i
   XTB_CHECK_ARG(T >= 0 && H > 0 && E > 0 && K > 0 && K <= E, "xtb_gate_route_dispatch: bad shape T=%d H=%d E=%d K=%d", T,
                 H, E, K);
   XTB_CHECK_ARG(E <= 8 && K <= 8 && H % 128 == 0 && (size_t)48 * H <= 200 * 1024,
-                "xtb_gate_route_dispatch: supports E <= 8, H %% 128 == 0, H <= 4096 (got E=%d H=%d); use xtb_gate_logits + "
+                "xtb_gate_route_dispatch: supports E <= 8, H %% 128 == 0, H <= 4224 (got E=%d H=%d); use xtb_gate_logits + "
                 "xtb_router_greedy_dispatch",
                 E, H);
   XTB_ENSURE_CTX(x_bf16);

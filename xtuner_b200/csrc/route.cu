@@ -435,8 +435,12 @@ router_greedy_kernel(const float* __restrict__ logits, int T, int E, int K, int 
       }
     }
     group_argmax<LPT, VPL>(bv, be);
-    if (be < 0 || be >= E) {  // only reachable with NaN rows: stay in range (lowest free index)
-      be = k;
+    if (be < 0 || be >= E) {  // only reachable with NaN rows: the lowest index not selected yet.  sel_e is the same on
+                              // every lane of the group, and that index is at most k < K <= E.
+      unsigned used = 0;
+      for (int i = 0; i < k; ++i)
+        if (sel_e[i] < 32) used |= 1u << sel_e[i];
+      be = __ffs(~used) - 1;
       bv = 0.f;
     }
     if (be >= e0 && be < e0 + VPL) taken |= 1u << (be - e0);
@@ -639,6 +643,14 @@ __global__ void __launch_bounds__(256) router_noaux_kernel(const float* __restri
       const float ow = __shfl_xor_sync(0xffffffffu, bw, o);
       if (ov > bv || (ov == bv && oe < be)) { bv = ov; be = oe; bw = ow; }
     }
+    if (be < 0 || be >= E) {  // no score left that compares (NaN or -inf): the lowest index not selected yet, with
+                              // weight 0.  sel_e is the same on every lane, and that index is at most k < K <= E.
+      unsigned used = 0;
+      for (int i = 0; i < k; ++i)
+        if (sel_e[i] < 32) used |= 1u << sel_e[i];
+      be = __ffs(~used) - 1;
+      bw = 0.f;
+    }
     if (be >= e0 && be < e0 + VPL) taken |= 1u << (be - e0);
     if (k < 32) { sel_w[k] = bw; sel_e[k] = be; }
     sum += bw;
@@ -660,14 +672,73 @@ __global__ void __launch_bounds__(256) router_noaux_kernel(const float* __restri
     if (s_hist[i]) atomicAdd(&tokens_per_expert[i], (float)s_hist[i]);  // exact: integer counts < 2^24
 }
 
+// Which of a token's experts the no-aux router's group mask keeps, recomputed from the choice scores ch = s + b.  A
+// group's score is its exact largest plus its exact second largest choice score, and topk_group rounds of
+// (score desc, group index asc) pick the kept groups; both are independent of how the experts are spread over lanes,
+// so this gives router_noaux_kernel's choice under any lane mapping.  LPT lanes hold VPL consecutive experts each;
+// groups of gs = E / n_group experts (a power of two) either lie whole inside one lane (gs <= VPL) or span gs / VPL
+// neighbouring lanes.  The router weight of a kept expert may be exactly 0 (s + b == 0), so router_weights cannot
+// tell kept from masked experts.
+template <int LPT, int VPL>
+__device__ __forceinline__ void noaux_kept_experts(const float (&ch)[VPL], int e0, int E, int n_group, int topk_group,
+                                                   bool (&keep)[VPL]) {
+  const int gs = E / n_group;
+  // gv[j]: score of the group whose last local expert is j (candidate slots); others -inf and not candidates
+  float gv[VPL];
+  bool cand[VPL];
+  float a = -INFINITY, b = -INFINITY;  // a >= b: top two of the current group
+#pragma unroll
+  for (int j = 0; j < VPL; ++j) {
+    const float v = ch[j];
+    if (v > a) { b = a; a = v; } else if (v > b) { b = v; }
+    const bool last = gs <= VPL && ((j + 1) % gs == 0);
+    gv[j] = last ? a + b : -INFINITY;
+    cand[j] = last;
+    if (last) a = b = -INFINITY;
+  }
+  if (gs > VPL) {  // merge the top-2 pairs of the gs / VPL lanes of the group; its first lane holds the candidate
+    for (int o = 1; o < gs / VPL; o <<= 1) {
+      const float oa = __shfl_xor_sync(0xffffffffu, a, o);
+      const float ob = __shfl_xor_sync(0xffffffffu, b, o);
+      const float na = fmaxf(a, oa);
+      const float nb = fmaxf(fminf(a, oa), fmaxf(b, ob));
+      a = na;
+      b = nb;
+    }
+    gv[VPL - 1] = a + b;
+    cand[VPL - 1] = (e0 % gs) == 0;
+  }
+  unsigned kept = 0;  // bit g: group g kept (n_group <= 32); the same on every lane of the token
+  for (int r = 0; r < topk_group; ++r) {
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+#pragma unroll
+    for (int j = 0; j < VPL; ++j) {
+      const int gi = (e0 + j) / gs;
+      if (cand[j] && !((kept >> gi) & 1u) && (gv[j] > bv || (gv[j] == bv && gi < bi))) {
+        bv = gv[j];
+        bi = gi;
+      }
+    }
+#pragma unroll
+    for (int o = LPT / 2; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+    if (bi < n_group) kept |= 1u << bi;
+  }
+#pragma unroll
+  for (int j = 0; j < VPL; ++j) keep[j] = (kept >> ((e0 + j) / gs)) & 1u;
+}
+
 // backward of the no-aux router (closed form: oracle/moe_oracle.py noaux_router_bwd).  LPT lanes per token, each
-// holding VPL consecutive experts.  The group mask is read back from the forward output: masked choice scores
-// are exactly 0 after masked_fill (noaux_router.py:113), so router_weights != 0 <=> the expert's group was kept.
+// holding VPL consecutive experts.  The group mask is recomputed from logits and bias (noaux_kept_experts).
 template <int LPT, int VPL>
 __global__ void __launch_bounds__(256) router_noaux_bwd_kernel(
     const float* __restrict__ logits, const float* __restrict__ bias, const float* __restrict__ router_weights,
     const float* __restrict__ topk_weights, const int64_t* __restrict__ topk_ids, const float* __restrict__ g_tw,
-    const float* __restrict__ g_rw, int T, int E, int K, int has_group_mask, int norm_topk, float scaling,
+    const float* __restrict__ g_rw, int T, int E, int K, int n_group, int topk_group, int norm_topk, float scaling,
     float* __restrict__ grad_logits) {
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x;
   const int token = gtid / LPT;
@@ -688,12 +759,21 @@ __global__ void __launch_bounds__(256) router_noaux_bwd_kernel(
     // r = c / S with c = mask * (s + b):  dc_j = mask_j * (g_j - sum_i g_i r_i) / S
     float S = 0.f, dot = 0.f, g[VPL];
     bool keep[VPL];
+    if (n_group != topk_group) {
+      float ch[VPL];
+#pragma unroll
+      for (int j = 0; j < VPL; ++j) ch[j] = (e0 + j < E) ? sg[j] + bias[e0 + j] : -INFINITY;
+      noaux_kept_experts<LPT, VPL>(ch, e0, E, n_group, topk_group, keep);
+    } else {
+#pragma unroll
+      for (int j = 0; j < VPL; ++j) keep[j] = true;
+    }
 #pragma unroll
     for (int j = 0; j < VPL; ++j) {
       const int e = e0 + j;
       const float r = (e < E) ? router_weights[(size_t)tok * E + e] : 0.f;
       g[j] = (e < E) ? g_rw[(size_t)tok * E + e] : 0.f;
-      keep[j] = (e < E) && (!has_group_mask || r != 0.f);
+      keep[j] = keep[j] && (e < E);
       if (keep[j]) S += sg[j] + bias[e];
       dot = fmaf(g[j], r, dot);
     }
@@ -905,11 +985,11 @@ static int launch_router_greedy_bwd(const float* rw, const float* tw, const int6
 template <int LPT, int VPL>
 static int launch_router_noaux_bwd(const float* logits, const float* bias, const float* rw, const float* tw,
                                    const int64_t* ids, const float* g_tw, const float* g_rw, int T, int E, int K,
-                                   int has_mask, int norm, float scaling, float* gl, cudaStream_t st) {
+                                   int n_group, int topk_group, int norm, float scaling, float* gl, cudaStream_t st) {
   const int tokens_per_block = 256 / LPT;
   const int blocks = (T + tokens_per_block - 1) / tokens_per_block;
-  router_noaux_bwd_kernel<LPT, VPL><<<blocks, 256, 0, st>>>(logits, bias, rw, tw, ids, g_tw, g_rw, T, E, K, has_mask,
-                                                           norm, scaling, gl);
+  router_noaux_bwd_kernel<LPT, VPL><<<blocks, 256, 0, st>>>(logits, bias, rw, tw, ids, g_tw, g_rw, T, E, K, n_group,
+                                                           topk_group, norm, scaling, gl);
   XTB_LAUNCH_OK();
   return XTB_OK;
 }
@@ -1004,16 +1084,27 @@ extern "C" int xtb_router_noaux(const float* logits, const float* e_score_correc
 extern "C" int xtb_router_noaux_bwd(const float* logits, const float* e_score_correction_bias,
                                     const float* router_weights, const float* topk_weights, const int64_t* topk_ids,
                                     const float* grad_topk_weights, const float* grad_router_weights, int T, int E,
-                                    int K, int has_group_mask, int norm_topk_prob, float scaling, float* grad_logits,
+                                    int K, int group_spec, int norm_topk_prob, float scaling, float* grad_logits,
                                     xtb_stream_t stream) {
   XTB_CHECK_ARG(logits && e_score_correction_bias && router_weights && topk_weights && topk_ids && grad_logits,
                 "xtb_router_noaux_bwd: null pointer");
   XTB_CHECK_ARG(T >= 0 && E > 0 && K > 0 && K <= E, "xtb_router_noaux_bwd: bad shape T=%d E=%d K=%d", T, E, K);
+  // group_spec = XTB_NOAUX_GROUP_SPEC(n_group, topk_group); 0: no group mask
+  const int n_group = group_spec ? (group_spec & 0xFF) : 1;
+  const int topk_group = group_spec ? (group_spec >> 8) : 1;
+  if (group_spec) {  // the forward's geometry (xtb_router_noaux): every group lies in one lane or spans 2^i lanes
+    XTB_CHECK_ARG(E % 32 == 0 && E <= 512, "xtb_router_noaux_bwd: E=%d must be a multiple of 32 and <= 512", E);
+    XTB_CHECK_ARG(n_group >= 1 && n_group <= 32 && E % n_group == 0 && topk_group >= 1 && topk_group < n_group,
+                  "xtb_router_noaux_bwd: bad group_spec %d (n_group=%d, topk_group=%d)", group_spec, n_group, topk_group);
+    XTB_CHECK_ARG(((E / n_group) & (E / n_group - 1)) == 0 && (E / n_group) % (E / 32) == 0,
+                  "xtb_router_noaux_bwd: group size %d must be a power of two and a multiple of E/32=%d", E / n_group,
+                  E / 32);
+  }
   XTB_ENSURE_CTX(logits);
   if (T == 0) return XTB_OK;
   cudaStream_t st = as_stream(stream);
   XTB_ROUTER_DISPATCH(launch_router_noaux_bwd, logits, e_score_correction_bias, router_weights, topk_weights, topk_ids,
-                      grad_topk_weights, grad_router_weights, T, E, K, has_group_mask, norm_topk_prob, scaling,
+                      grad_topk_weights, grad_router_weights, T, E, K, n_group, topk_group, norm_topk_prob, scaling,
                       grad_logits, st)
 }
 

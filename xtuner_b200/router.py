@@ -188,10 +188,16 @@ def _(logits, bias, top_k, n_group, topk_group, norm_topk_prob, scaling):
     )
 
 
+def noaux_group_spec(n_group: int, topk_group: int) -> int:
+    """The ``group_spec`` argument of xtb_router_noaux_bwd (XTB_NOAUX_GROUP_SPEC in the header): 0 without a group
+    mask, else n_group | topk_group << 8."""
+    return 0 if n_group == topk_group else n_group | (topk_group << 8)
+
+
 @torch.library.custom_op("xtuner_b200::router_noaux_bwd", mutates_args=())
 def _router_noaux_bwd_op(
     logits: Tensor, bias: Tensor, rw: Tensor, tw: Tensor, ids: Tensor, g_tw: Optional[Tensor], g_rw: Optional[Tensor],
-    has_group_mask: bool, norm_topk_prob: bool, scaling: float,
+    group_spec: int, norm_topk_prob: bool, scaling: float,
 ) -> Tensor:
     lib = _capi.ensure_init()
     T, E = logits.shape
@@ -199,7 +205,7 @@ def _router_noaux_bwd_op(
     check(
         lib.xtb_router_noaux_bwd(
             ptr(logits), ptr(bias), ptr(rw), ptr(tw), ptr(ids), ptr(g_tw), ptr(g_rw), T, E, tw.shape[1],
-            int(has_group_mask), int(norm_topk_prob), float(scaling), ptr(gl), current_stream(),
+            group_spec, int(norm_topk_prob), float(scaling), ptr(gl), current_stream(),
         ),
         "xtb_router_noaux_bwd",
     )
@@ -207,7 +213,7 @@ def _router_noaux_bwd_op(
 
 
 @_router_noaux_bwd_op.register_fake
-def _(logits, bias, rw, tw, ids, g_tw, g_rw, has_group_mask, norm_topk_prob, scaling):
+def _(logits, bias, rw, tw, ids, g_tw, g_rw, group_spec, norm_topk_prob, scaling):
     return torch.empty_like(logits)
 
 
@@ -219,17 +225,17 @@ class _NoAuxRoute(torch.autograd.Function):
     def forward(ctx, logits, bias, top_k, n_group, topk_group, norm, scaling):
         rw, tw, ids, ids32, tpe = _router_noaux_op(logits, bias, top_k, n_group, topk_group, norm, scaling)
         ctx.save_for_backward(logits, bias, rw, tw, ids)
-        ctx.cfg = (n_group != topk_group, norm, scaling)
+        ctx.cfg = (noaux_group_spec(n_group, topk_group), norm, scaling)
         ctx.mark_non_differentiable(ids, ids32, tpe)
         return rw, tw, ids, ids32, tpe
 
     @staticmethod
     def backward(ctx, g_rw, g_tw, _a, _b, _c):
         logits, bias, rw, tw, ids = ctx.saved_tensors
-        has_mask, norm, scaling = ctx.cfg
+        group_spec, norm, scaling = ctx.cfg
         g_rw = None if g_rw is None else g_rw.contiguous()
         g_tw = None if g_tw is None else g_tw.contiguous()
-        gl = _router_noaux_bwd_op(logits, bias, rw, tw, ids, g_tw, g_rw, has_mask, norm, scaling)
+        gl = _router_noaux_bwd_op(logits, bias, rw, tw, ids, g_tw, g_rw, group_spec, norm, scaling)
         return gl, None, None, None, None, None, None
 
 
