@@ -306,7 +306,8 @@ int xtb_allreduce_pull_f32(void* const* peer_in_ptrs_dev, void* out, int rank, i
 
 /* Batch of device-to-device copies between (peer-mapped) addresses on the copy engines — the FSDP engine's XTB_FSDP_DMA
  * mode moves the gathered parameters / gradient slices with it so that no SM is taken from the GEMMs it runs under.
- * All three arrays are HOST arrays of length n; entries with nbytes == 0 or dst == src are skipped. */
+ * All three arrays are HOST arrays of length n; entries with nbytes == 0 or dst == src are skipped.  Every entry is
+ * checked before anything is enqueued: a batch with a bad entry is refused without copying any entry. */
 int xtb_peer_memcpy_batch(void* const* dst_ptrs_host, const void* const* src_ptrs_host, const int64_t* nbytes_host, int n,
                           xtb_stream_t stream);
 

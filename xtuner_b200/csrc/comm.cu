@@ -297,9 +297,11 @@ extern "C" int xtb_peer_memcpy_batch(void* const* dst_ptrs_host, const void* con
                                      const int64_t* nbytes_host, int n, xtb_stream_t stream) {
   XTB_CHECK_ARG(dst_ptrs_host && src_ptrs_host && nbytes_host, "xtb_peer_memcpy_batch: null pointer");
   XTB_CHECK_ARG(n >= 0 && n <= 4096, "xtb_peer_memcpy_batch: bad n=%d", n);
+  // every entry is checked before the first copy is enqueued: a refused batch copies nothing
+  for (int i = 0; i < n; ++i)
+    XTB_CHECK_ARG(dst_ptrs_host[i] && src_ptrs_host[i] && nbytes_host[i] >= 0, "xtb_peer_memcpy_batch: bad entry %d", i);
   cudaStream_t st = as_stream(stream);
   for (int i = 0; i < n; ++i) {
-    XTB_CHECK_ARG(dst_ptrs_host[i] && src_ptrs_host[i] && nbytes_host[i] >= 0, "xtb_peer_memcpy_batch: bad entry %d", i);
     if (nbytes_host[i] == 0 || dst_ptrs_host[i] == src_ptrs_host[i]) continue;
     XTB_ENSURE_CTX(src_ptrs_host[i]);
     XTB_CUDA(cudaMemcpyAsync(dst_ptrs_host[i], src_ptrs_host[i], (size_t)nbytes_host[i], cudaMemcpyDeviceToDevice, st));
