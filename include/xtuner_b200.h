@@ -80,12 +80,14 @@ int xtb_router_greedy_dispatch(const float* logits, int T, int E, int K, int sco
                                float scaling, float* router_weights, float* topk_weights, int64_t* topk_ids,
                                int32_t* topk_ids_i32, int64_t* tokens_per_expert, void* dispatch_workspace,
                                xtb_stream_t stream);
-/* a1 + a2 + the index half of a4 in ONE launch (csrc/gate_mma.cu) — what the fused layer calls; bit-equal on an H100 to the two
- * calls it stands for when they use the same tensor-core gate (tests/test_gpu_router.py).  Gate logits on
- * the tensor cores (fp32 weight as three bf16 planes, exact products, fp32 accumulation), then the greedy router of
+/* a1 + a2 + the index half of a4 in ONE launch (csrc/gate_mma.cu) — what the fused layer calls.  Gate logits on the
+ * tensor cores (fp32 weight as three bf16 planes, exact products, fp32 accumulation), then the greedy router of
  * xtb_router_greedy_dispatch on the 32-token block that is still in shared memory, then the chunk histograms and their
- * scan: same outputs as xtb_gate_logits (no bias) followed by xtb_router_greedy_dispatch, one kernel instead of two and
- * no logits round trip.  E <= 8, K <= 8, H % 128 == 0, H <= 4096; XTB_ERR_INVALID otherwise (use the two calls). */
+ * scan: the outputs of xtb_gate_logits (no bias) followed by xtb_router_greedy_dispatch, one kernel instead of two and
+ * no logits round trip.  The logits equal float64 on exact inputs and stay within the bound of
+ * tests/router_reference.py otherwise; every other output, the dispatch workspace included, is bit-equal on an H100 to
+ * xtb_router_greedy_dispatch run on those logits (tests/test_gpu_router_edges.py).  E <= 8, K <= 8, H % 128 == 0,
+ * H <= 4224; XTB_ERR_INVALID otherwise (use the two calls). */
 int xtb_gate_route_dispatch(const void* x_bf16, const float* w_f32, int T, int H, int E, int K, int scoring,
                             int norm_topk_prob, float scaling, float* logits, float* router_weights,
                             float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32, int64_t* tokens_per_expert,
@@ -99,7 +101,7 @@ int xtb_router_greedy_bwd(const float* router_weights, const float* topk_weights
                           float scaling, float* grad_logits, xtb_stream_t stream);
 
 /* backward of a2 and of a1 in ONE launch — what the fused layer calls; bit-equal on an H100 to xtb_router_greedy_bwd +
- * xtb_gate_logits_bwd (tests/test_gpu_router.py): grad_logits is computed per token in the
+ * xtb_gate_logits_bwd (tests/test_gpu_router_edges.py): grad_logits is computed per token in the
  * prologue of the gate backward (same formula and order as xtb_router_greedy_bwd) and never written to memory;
  * grad_w / grad_x as xtb_gate_logits_bwd (no bias).  workspace: xtb_gate_logits_bwd_workspace_bytes(T, H, E).
  * E <= 8, H % 8 == 0; XTB_ERR_INVALID otherwise (use the two calls). */
@@ -151,9 +153,6 @@ int xtb_moe_permute(const void* x, const int32_t* ids, int T, int K, int E, int6
 int xtb_moe_permute_prepared(const void* x, const int32_t* ids, int T, int K, int E, int64_t row_bytes,
                              void* permuted, int32_t* row_id_map, int64_t* sorted_indices,
                              const void* prepared_workspace, xtb_stream_t stream);
-/* Only the index work of a4 (no row copy): used when the gather is fused into a consumer. */
-int xtb_moe_permute_index(const int32_t* ids, int T, int K, int E, int32_t* row_id_map, int64_t* sorted_indices,
-                          int64_t* tokens_per_expert, void* workspace, xtb_stream_t stream);
 
 /* ---- a5  unpermute: ops/moe/protocol.py:26-30, permute_unpermute.py:146-192,222-248 ----------------
  * out[t] = bf16( sum_k fp32(probs[t,k]) * fp32(y[row_id_map[t*K+k]]) ), fp32 accumulation in k order.

@@ -58,7 +58,6 @@ KERNELS = {
     "router_greedy": (lambda i: lib.xtb_router_greedy(ptr(logits[i]), T, E, K, 0, 1, 1.0, ptr(rw), ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), st), T * E * 8, "B"),
     "router_greedy_bwd": (lambda i: lib.xtb_router_greedy_bwd(ptr(rw), ptr(tw), ptr(ids), ptr(gtw), None, None, T, E, K, 0, 1, 1.0, ptr(logits[i]), st), T * E * 8, "B"),
     "permute": (lambda i: lib.xtb_moe_permute(ptr(xs[i]), ptr(ids32), T, K, E, H * 2, ptr(xperm[i]), ptr(rmap), None, None, ptr(ws), st), B_perm, "B"),
-    "permute_index": (lambda i: lib.xtb_moe_permute_index(ptr(ids32), T, K, E, ptr(rmap), None, None, ptr(ws), st), T * K * 8, "B"),
     "combine": (lambda i: lib.xtb_moe_combine(ptr(ys[i]), ptr(rmap), ptr(tw), None, 1.0, T, K, H, ptr(outs[i]), st), B_perm, "B"),
     "combine_residual": (lambda i: lib.xtb_moe_combine(ptr(ys[i]), ptr(rmap), ptr(tw), ptr(xs[i]), 1.0, T, K, H, ptr(outs[i]), st), B_perm + T * H * s, "B"),
     "unpermute_bwd": (lambda i: lib.xtb_moe_unpermute_bwd(ptr(xs[i]), ptr(ys[i]), ptr(rmap), ptr(tw), T, K, H, ptr(xperm[i]), ptr(gtw), st), T * H * s + 2 * M * H * s, "B"),

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Compares the SASS instruction stream of every kernel in two builds of libxtuner_b200.so (function by function,
-addresses stripped).  Used to show that adding opt-in template variants left the GPU-validated default kernels
+addresses stripped).  Used to show that adding or removing template variants left the GPU-validated default kernels
 untouched:   python scripts/sass_compare.py OLD.so NEW.so"""
 import subprocess, re, hashlib, sys
 def funcs(lib):
@@ -9,16 +9,19 @@ def funcs(lib):
     for line in out.splitlines():
         m=re.search(r"Function : (\S+)", line)
         if m: cur=m.group(1); res[cur]=[]; continue
-        m=re.match(r"\s+/\*[0-9a-f]{4}\*/\s+(.*?);", line)
+        m=re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?);", line)
         if m and cur: res[cur].append(m.group(1).strip())
     return res
 old=funcs(sys.argv[1]); new=funcs(sys.argv[2])
 def demangle(n): return subprocess.run(["c++filt",n],capture_output=True,text=True).stdout.strip().split("(")[0]
 newd={demangle(k):k for k in new}
+def dropped(d):  # a template parameter removed together with its other value: <M, N, E, 1> -> <M, N, E>, f<true> -> f
+    d=re.sub(r"<(\d+), (\d+), (\d+), 1>$", r"<\1, \2, \3>", d)
+    return re.sub(r"^void (\S+)<true>$", r"\1", d)
 same=diff=0
 for k,v in old.items():
     d=demangle(k)
-    cands=[nk for nd,nk in newd.items() if nd==d or nd.replace(", false>",">")==d or nd.replace(", (bool)0>",">")==d]
+    cands=[nk for nd,nk in newd.items() if nd in (d, dropped(d)) or nd.replace(", false>",">")==d or nd.replace(", (bool)0>",">")==d]
     if not cands:
         print("MISSING in new:", d); continue
     nv=new[cands[0]]

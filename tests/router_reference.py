@@ -8,11 +8,11 @@ gamma(n) = n u / (1 - n u) bound n successive fp32 roundings of a sum whose part
   ``small``    gate_logits_small_kernel: each lane chains H/32 fmaf (8 per 256-column chunk), a 5-level warp tree adds
                the 32 lane sums, the bias adds once: gamma(H/32 + 6) (S + |b|).
   ``strided``  sgemm_strided_kernel: one chain of H fmaf per output, then the bias: gamma(H + 1) (S + |b|).
-  ``mma``      gate_logits_mma_kernel and the fused gate: w = hi + mid + lo exactly (three bf16 planes, 24 bits), every
-               bf16 product is exact in fp32, and each K quarter runs 6 H/128 m16n8k16 steps into one fp32 accumulator;
-               the four quarters are added in order, then the bias.  The tensor core's internal accumulation is not
-               assumed to round to nearest: each step is allowed 2u (truncation) relative to the partial sums, so
-               2 gamma(6 H/128) + gamma(4) on S, + |b| gamma(1).
+  ``mma``      the tensor-core gate of xtb_gate_route_dispatch: w = hi + mid + lo exactly (three bf16 planes, 24
+               bits), every bf16 product is exact in fp32, and each K quarter runs 6 H/128 m16n8k16 steps into one fp32
+               accumulator; the four quarters are added in order, then the bias.  The tensor core's internal
+               accumulation is not assumed to round to nearest: each step is allowed 2u (truncation) relative to the
+               partial sums, so 2 gamma(6 H/128) + gamma(4) on S, + |b| gamma(1).
 
 Input modes for the gate (:func:`gate_inputs`):
 

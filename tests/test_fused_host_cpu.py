@@ -2,8 +2,8 @@
 nodes run forward+backward against ``tests/cabi_emulator.EmulatedLib`` (host-memory emulation of the C-ABI, written from
 the header's contract) and must agree with the oracle under torch autograd.  What this pins: buffer shapes/dtypes,
 argument order at every call, the backward chain (which saved tensor feeds which product, where gradients are
-summed), optional paths (no residual, norm-weight grad not needed, fused vs separate gate/router entry points).  The kernels themselves are
-covered by the `-m gpu` parity tests."""
+summed), optional paths (no residual, norm-weight grad not needed, one-launch vs separate gate/router entry points by
+shape).  The kernels themselves are covered by the `-m gpu` parity tests."""
 import pytest
 import torch
 from torch.nn import functional as F
@@ -218,49 +218,39 @@ def test_op_protocol_permute_unpermute_on_reference_fixtures(emu, monkeypatch, t
     assert ge.shape == (0, 128) and ge.requires_grad
 
 
+@pytest.mark.parametrize("E", [8, 16])
 @pytest.mark.parametrize("block", [False, True])
-def test_gate_route_fused_flag_wiring(emu, monkeypatch, block):
-    """XTB_GATE_ROUTE_FUSED: one call replaces gate + router in both fused nodes; results unchanged."""
+def test_route_entry_points_follow_the_shape(emu, block, E):
+    """Both fused nodes at H = 128: E = 8 runs the gate + router forward as xtb_gate_route_dispatch and the router + gate
+    backward as xtb_router_gate_bwd, E = 16 the separate calls each of them replaces.  Outputs and gradients against
+    the oracle either way."""
     from xtuner_b200 import fused
 
-    T, H, I, E, K = 64, 128, 256, 8, 2
-    h, gate_w, w13, w2, g_out, _a, _b = _weights(T, H, I, E, 5)
-    outs = []
-    for flag in (False, True):
-        monkeypatch.setattr(fused, "GATE_ROUTE_FUSED", flag)
-        emu.calls.clear()
-        hr = h.clone().requires_grad_(True)
-        if block:
-            out, logits, rw, ids, tpe = fused.FusedMoEBlockFunction.apply(hr, torch.ones(H), 1e-6, gate_w, w13, w2, K, True, 1.0, 1.0, 0)
-        else:
-            out, logits, rw, ids, tpe = fused.FusedMoEFunction.apply(hr, None, gate_w, w13, w2, K, True, 1.0, 1.0, 0)
-        (gh,) = torch.autograd.grad(out, hr, g_out)
-        outs.append((out, logits, rw, ids, tpe, gh))
-        assert ("xtb_gate_route_dispatch" in emu.calls) == flag
-        assert ("xtb_router_greedy_dispatch" in emu.calls) == (not flag) and ("xtb_gate_logits" in emu.calls) == (not flag)
-    for a, b in zip(*outs):
-        assert torch.equal(a, b)
+    T, H, I, K, eps = 64, 128, 256, 2, 1e-6
+    h, gate_w, w13, w2, g_out, g_rw, g_lg = _weights(T, H, I, E, 5)
+    norm_w = 1.0 + 0.1 * torch.randn(H, generator=torch.Generator().manual_seed(E))
 
+    hr, gr = (t.clone().requires_grad_(True) for t in (h, gate_w))
+    x = F.rms_norm(hr.float(), (H,), norm_w, eps).to(torch.bfloat16) if block else hr
+    ref = O.moe_layer_forward(x, gr, w13, w2, K, True, 1.0, 1.0, residual=hr if block else None)
+    ref_grads = torch.autograd.grad([ref["hidden_states"], ref["router.router_weights"], ref["router.logits"]], [hr, gr],
+                                    [g_out, g_rw, g_lg])
 
-@pytest.mark.parametrize("block", [False, True])
-def test_router_gate_bwd_fused_flag_wiring(emu, monkeypatch, block):
-    """XTB_ROUTER_GATE_BWD_FUSED: one call replaces router-bwd + gate-bwd in both fused nodes; gradients unchanged."""
-    from xtuner_b200 import fused
+    emu.calls.clear()
+    ho, go = (t.clone().requires_grad_(True) for t in (h, gate_w))
+    if block:
+        out, logits, rw, ids, tpe = fused.FusedMoEBlockFunction.apply(ho, norm_w, eps, go, w13, w2, K, True, 1.0, 1.0, 0)
+    else:
+        out, logits, rw, ids, tpe = fused.FusedMoEFunction.apply(ho, None, go, w13, w2, K, True, 1.0, 1.0, 0)
+    grads = torch.autograd.grad([out, rw, logits], [ho, go], [g_out, g_rw, g_lg])
 
-    T, H, I, E, K = 64, 128, 256, 8, 2
-    h, gate_w, w13, w2, g_out, g_rw, g_lg = _weights(T, H, I, E, 6)
-    res = []
-    for flag in (False, True):
-        monkeypatch.setattr(fused, "ROUTER_GATE_BWD_FUSED", flag)
-        emu.calls.clear()
-        hr = h.clone().requires_grad_(True)
-        gw = gate_w.clone().requires_grad_(True)
-        if block:
-            out, logits, rw, ids, tpe = fused.FusedMoEBlockFunction.apply(hr, torch.ones(H), 1e-6, gw, w13, w2, K, True, 1.0, 1.0, 0)
-        else:
-            out, logits, rw, ids, tpe = fused.FusedMoEFunction.apply(hr, None, gw, w13, w2, K, True, 1.0, 1.0, 0)
-        res.append(torch.autograd.grad([out, rw, logits], [hr, gw], [g_out, g_rw, g_lg]))
-        assert ("xtb_router_gate_bwd" in emu.calls) == flag
-        assert ("xtb_router_greedy_bwd" in emu.calls) == (not flag) and ("xtb_gate_logits_bwd" in emu.calls) == (not flag)
-    for a, b in zip(*res):
-        assert torch.equal(a, b)
+    one_launch = {"xtb_gate_route_dispatch", "xtb_router_gate_bwd"}
+    split = {"xtb_gate_logits", "xtb_router_greedy_dispatch", "xtb_router_greedy_bwd", "xtb_gate_logits_bwd"}
+    called = set(emu.calls)
+    want, unwanted = (one_launch, split) if E <= 8 else (split, one_launch)
+    assert want <= called and not (unwanted & called), sorted(called)
+    assert torch.equal(ids, ref["router.topk_ids"]) and torch.equal(tpe, ref["tokens_per_expert"])
+    _close(out, ref["hidden_states"], "hidden_states")
+    torch.testing.assert_close(logits, ref["router.logits"], rtol=1e-5, atol=1e-5)
+    for name, a, b in zip(["h" if block else "x", "gate_w"], grads, ref_grads):
+        _close(a, b, f"grad {name}", tol=5e-2)

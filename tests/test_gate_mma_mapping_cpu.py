@@ -1,9 +1,9 @@
-"""Lane-level model of ``csrc/gate_mma.cu`` (the tensor-core gate inside ``xtb_gate_route_dispatch``; standalone with XTB_GATE_V=2).  The CUDA kernel cannot run in
-the CPU suite; this re-states its index arithmetic line by line — weight split into bf16 planes in B-fragment order,
+"""Lane-level model of ``csrc/gate_mma.cu`` (the tensor-core gate inside ``xtb_gate_route_dispatch``).  The CUDA kernel
+cannot run in the CPU suite; this re-states its index arithmetic line by line — weight split into bf16 planes in B-fragment order,
 per-lane 16-byte loads of x, the K permutation inside a 32-column block, the PTX fragment layout of
 mma.sync.m16n8k16 (row.col, bf16), the K-quarter reduction and the output mapping — and checks that the result is
-``x.float() @ w.T``.  It guards the mapping, not the hardware: the kernel's own parity test is
-tests/test_gpu_router.py::test_fused_gate_router_entry_points_equal_the_calls_they_replace."""
+``x.float() @ w.T``.  It guards the mapping, not the hardware: the kernel's own tests are
+tests/test_gpu_router_edges.py::test_fused_gate_logits and ::test_fused_gate_route_equals_router_on_its_own_logits."""
 import numpy as np
 import pytest
 import torch

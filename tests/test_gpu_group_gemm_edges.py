@@ -273,7 +273,8 @@ def test_more_than_1024_experts_is_rejected():
 
 def _expert_mlp_bounds(counts, H, I, seed):
     """Every entry at one expert-MLP geometry, random mode: the forward (nt_swiglu, then nt through w2), dX through both
-    weights (nn), both dW (tn and tn_pair); returns the largest |out - ref| / bound per product."""
+    weights (nn), both dW (tn, and tn_pair bit for bit against a tn launch per product); returns the largest
+    |out - ref| / bound per product."""
     E, M = len(counts), sum(counts)
     tpe = _tpe(counts)
     bf = dict(dtype=torch.bfloat16, device="cuda")
@@ -304,10 +305,14 @@ def _expert_mlp_bounds(counts, H, I, seed):
     gw2p, gw13p = torch.empty(E, H, I, **bf), torch.empty(E, 2 * I, H, **bf)
     _ok(tn_pair(dy, a, gw2p, dh, x, gw13p, tpe, E), "tn_pair")
     torch.cuda.synchronize()
-    assert torch.equal(gw2p.view(torch.int16), gw2.view(torch.int16)), "tn_pair differs from tn"
+    assert torch.equal(gw2p.view(torch.int16), gw2.view(torch.int16)), "tn_pair differs from tn (gw2)"
     del gw2, gw2p
     ratios["tn_pair"] = R.check_bound(gw13p, "tn", dh, x, counts, what="gw13 pair")
-    del gw13p
+    gw13 = torch.empty(E, 2 * I, H, **bf)
+    _ok(tn(dh, x, tpe, gw13, E), "tn w13")
+    torch.cuda.synchronize()
+    assert torch.equal(gw13p.view(torch.int16), gw13.view(torch.int16)), "tn_pair differs from tn (gw13)"
+    del gw13, gw13p
     return ratios, dict(x=x, w13=w13, w2=w2, a=a, dy=dy, tpe=tpe)
 
 

@@ -172,58 +172,3 @@ def test_greedy_router_variants_golden(tag):
     (gl,) = torch.autograd.grad([res["topk_weights"], res["router_weights"]], lg,
                                 [g["grad_topk_weights"].cuda(), g["grad_router_weights"].cuda()])
     torch.testing.assert_close(gl.cpu(), g["grad_logits"], rtol=1e-4, atol=1e-6)
-
-
-def _gate_worker(tmp_path, tag, **env_extra):
-    import os
-    import subprocess
-    import sys
-
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    path = str(tmp_path / f"gate_{tag}.pt")
-    env = dict(os.environ, PYTHONPATH=root + os.pathsep + os.environ.get("PYTHONPATH", ""), **env_extra)
-    r = subprocess.run([sys.executable, os.path.join(root, "tests", "workers", "gate_worker.py"), path], env=env, cwd=root,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return torch.load(path)
-
-
-def _gate_w(key):
-    _tag, T, H, E = key
-    g = torch.Generator().manual_seed(7 * T + E)
-    torch.randn(T, H, generator=g)
-    torch.randn(H, generator=g)
-    return torch.randn(E, H, generator=g) * 0.05
-
-
-def test_fused_gate_router_entry_points_equal_the_calls_they_replace(tmp_path):
-    """The two one-launch entry points of the fused layer's default path against the separate calls, bit for bit:
-    xtb_gate_route_dispatch == xtb_gate_logits (same tensor-core gate, XTB_GATE_V=2) + xtb_router_greedy_dispatch, including
-    the permuted rows the dispatch workspace leads to; xtb_router_gate_bwd == xtb_router_greedy_bwd + xtb_gate_logits_bwd.
-    And the tensor-core gate itself against the CUDA-core kernel and the oracle."""
-    outs = {"1": _gate_worker(tmp_path, "v1", XTB_GATE_V="1"), "2": _gate_worker(tmp_path, "v2", XTB_GATE_V="2")}
-    fused_keys = [k for k in outs["2"] if k[0] == "gate_route"]
-    assert fused_keys, "the worker did not run the gate+route comparison"
-    for key in fused_keys:
-        two, one = outs["2"][key]
-        for name in two:
-            assert torch.equal(two[name], one[name]), (key, name)
-    for run in outs.values():
-        keys = [k for k in run if k[0] == "router_gate_bwd"]
-        assert keys
-        for k in keys:
-            (gw1, gx1), (gw2, gx2) = run[k]
-            assert torch.equal(gw1, gw2) and torch.equal(gx1, gx2), k
-    for key in outs["1"]:
-        if not (len(key) == 4 and isinstance(key[0], int)):
-            continue
-        a, b = outs["1"][key], outs["2"][key]
-        assert torch.isfinite(b).all(), key
-        torch.testing.assert_close(b, a, rtol=1e-5, atol=2e-5, msg=lambda m, key=key: f"{key}: {m}")
-        T, H, E, with_bias = key
-        g = torch.Generator().manual_seed(T + E)
-        x = torch.randn(T, H, generator=g).to(torch.bfloat16)
-        w = torch.randn(E, H, generator=g) * 0.05
-        bias = torch.randn(E, generator=g) if with_bias else None
-        ref = O.gate_logits(x, w) + (bias if with_bias else 0)
-        torch.testing.assert_close(b, ref, rtol=1e-4, atol=1e-4)

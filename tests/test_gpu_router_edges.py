@@ -9,10 +9,12 @@ of tests/router_reference.py, at the edges the parity tests of tests/test_gpu_ro
   normalising on and off, scaling 1 and 2.5, with and without the dispatch workspace (chunk histograms and
   expert_start against a CPU scan).  Exact checks on the kernel's own router_weights, router_weights within the expf
   bound, ids equal to float64 on decided rows.  Tie rows, rows of tied zeros, NaN and +-inf rows.  Refusals.
-* Fused gate + route + dispatch bit-equal to xtb_router_greedy_dispatch on its own logits, E = 1 to 8, K = 1 to E.
+* Fused gate + route + dispatch bit-equal to xtb_router_greedy_dispatch on its own logits, and the rows
+  xtb_moe_permute_prepared gathers from either workspace bit-equal, at E = 1 to 8, K = 1 to E and at the benchmark
+  shape (T = 8192, H = 2048, E = 8, K = 2).
 * Backward: xtb_router_greedy_bwd against float64 autograd with every null combination of the three gradients;
-  xtb_router_gate_bwd bit-equal to the two calls it replaces at E = 1 to 8, K = 1 to E; the gate backward
-  (both small kernels, the strided pair, colsum) against float64 on both sides of 768 tokens per block.
+  xtb_router_gate_bwd bit-equal to the two calls it replaces at E = 1 to 8, K = 1 to E and at the benchmark shape; the
+  gate backward (both small kernels, the strided pair, colsum) against float64 on both sides of 768 tokens per block.
 * No-aux router: E = 32 to 512, K up to 32, lanes per group 1 to 8, no mask, tied group scores, negative-bias kept
   experts against masked zeros, the zero-score kept expert's gradient, NaN rows, refusals.
 * Determinism and T = 0.
@@ -200,16 +202,29 @@ def test_fused_gate_refuses_h_4352_and_accepts_4224():
     fused(x, w, 2, "softmax", True, 1.0)
 
 
-@pytest.mark.parametrize("E", range(1, 9))
-def test_fused_gate_route_equals_router_on_its_own_logits(E):
-    x, w, _ = R.gate_inputs(1000, 256, E, "random", E, "cuda")
-    for K in range(1, E + 1):
+def permute_prepared(x, ids32, ws, E):
+    """(permuted rows as int32 words, row_id_map) of xtb_moe_permute_prepared against a prepared workspace."""
+    T, H = x.shape
+    K = ids32.shape[1]
+    perm, rmap = Guarded(T * K, H // 2, torch.int32), Guarded(T, K, torch.int32)
+    _ok(_lib().xtb_moe_permute_prepared(_p(x), _p(ids32), T, K, E, H * 2, _p(perm.v), _p(rmap.v), None, _p(ws), _st()),
+        "xtb_moe_permute_prepared")
+    return perm.check("permuted"), rmap.check("row_id_map")
+
+
+@pytest.mark.parametrize("E,T,H,Ks", [pytest.param(E, 1000, 256, range(1, E + 1), id=str(E)) for E in range(1, 9)] + [
+    pytest.param(8, 8192, 2048, (2,), id="bench")])
+def test_fused_gate_route_equals_router_on_its_own_logits(E, T, H, Ks):
+    x, w, _ = R.gate_inputs(T, H, E, "random", E, "cuda")
+    for K in Ks:
         for scoring, norm, scaling in [("softmax", True, 1.0), ("sigmoid", False, 2.5), ("softmax", False, 2.5)]:
             f = fused(x, w, K, scoring, norm, scaling)
             r = router(f["logits"].clone(), K, scoring, norm, scaling, ws=True)
             for k in ("rw", "tw", "ids", "i32", "tpe", "ws"):
                 assert torch.equal(f[k].view(torch.uint8) if f[k].dtype == torch.float32 else f[k],
                                    r[k].view(torch.uint8) if r[k].dtype == torch.float32 else r[k]), (K, scoring, k)
+            (pf, mf), (pr, mr) = permute_prepared(x, f["i32"], f["ws"], E), permute_prepared(x, r["i32"], r["ws"], E)
+            assert torch.equal(mf, mr) and torch.equal(pf, pr), (K, scoring, "permuted rows")
 
 
 # ---- greedy router ---------------------------------------------------------------------------------------------------
@@ -322,13 +337,13 @@ def test_greedy_router_bwd(E):
                 _note("grad_logits (greedy)", R.check_bound(got[d], ref[d], bound[d], f"E={E} K={K} mask={mask}"))
 
 
-@pytest.mark.parametrize("E", range(1, 9))
-def test_router_gate_bwd_equals_the_two_calls(E):
+@pytest.mark.parametrize("E,T,H,Ks", [pytest.param(E, 1500, 256, range(1, E + 1), id=str(E)) for E in range(1, 9)] + [
+    pytest.param(8, 8192, 2048, (2,), id="bench")])
+def test_router_gate_bwd_equals_the_two_calls(E, T, H, Ks):
     lib = _lib()
-    T, H = 1500, 256
     x, w, _ = R.gate_inputs(T, H, E, "random", E, "cuda")
     lg = torch.randn(T, E, device="cuda")
-    for K in range(1, E + 1):
+    for K in Ks:
         scoring, norm, scaling = [("softmax", True, 1.0), ("sigmoid", False, 2.5)][K % 2]
         r = router(lg, K, scoring, norm, scaling)
         g_tw, g_rw, g_dir = torch.randn(T, K, device="cuda"), torch.randn(T, E, device="cuda"), torch.randn(T, E, device="cuda")

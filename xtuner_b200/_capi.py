@@ -68,7 +68,6 @@ SIGNATURES = {
     ),
     "xtb_moe_permute_prepared": (
         c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "xtb_moe_permute_index": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "xtb_moe_unpermute": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "xtb_moe_combine": (
         c_int,

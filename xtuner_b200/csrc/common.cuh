@@ -40,7 +40,6 @@ extern std::atomic<int64_t> g_launch_count;
 inline cudaStream_t as_stream(xtb_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 
 int sm_count();  // cached multiProcessorCount of the current device
-bool pdl_enabled();  // kernels of the fused MoE path launch with programmatic stream serialisation (XTB_PDL=0: off)
 
 // Binds a CUDA context to the calling thread if none is current (fresh autograd / worker threads have
 // none until their first runtime call), using the context that owns `device_ptr`.  Driver-API entry
@@ -61,7 +60,7 @@ int lm_head_logits_ce(const void* h, const void* w, const int64_t* tokens_per_ex
 // ---- device helpers ------------------------------------------------------------------------------
 #ifdef __CUDACC__
 
-// Programmatic dependent launch (default; XTB_PDL=0 switches it off).  A kernel launched through launch_pdl() may become resident while
+// Programmatic dependent launch.  A kernel launched through launch_pdl() may become resident while
 // its predecessor in the stream is still draining (its CTAs take over SMs as the predecessor's CTAs retire, hiding launch
 // latency and set-up); it must not touch global memory before pdl_sync().  Launched without the attribute, both
 // instructions are no-ops.
@@ -86,10 +85,6 @@ inline cudaError_t launch_pdl(void (*kernel)(P...), dim3 grid, dim3 block, size_
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  if (!pdl_enabled()) {  // the plain launch, exactly as before the switch existed
-    kernel<<<grid, block, smem, st>>>(P(args)...);
-    return cudaGetLastError();
-  }
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, P(args)...);

@@ -1,8 +1,7 @@
-// a1 (MoEGate.forward, moe_decoder_layer.py:120-141) on the tensor cores, and the one-launch gate + greedy router +
-// dispatch bucketing built on it (xtb_gate_route_dispatch: the default of the fused layer for E <= 8; fused against
-// two calls has not been measured on H100).  The stand-alone kernel (XTB_GATE_V=2 inside
-// xtb_gate_logits) is what the GPU test compares the fused launch with, bit for bit
-// (tests/test_gpu_router.py::test_gate_route_dispatch_equals_two_calls); fragment mapping modelled lane by lane on CPU
+// a1 (MoEGate.forward, moe_decoder_layer.py:120-141) on the tensor cores, fused with the greedy router and the dispatch
+// bucketing into one launch (xtb_gate_route_dispatch: the default of the fused layer for E <= 8; fused against two calls
+// has not been measured on H100).  tests/test_gpu_router_edges.py pins its logits against float64 and its routing and
+// bucketing bit for bit against the router run on those logits; the fragment mapping is modelled lane by lane on CPU
 // (tests/test_gate_mma_mapping_cpu.py).
 //
 // logits[T,E] = float(x[T,H]) @ float(w[E,H])^T for E <= 8.  The CUDA-core kernel (route.cu) is bound by shared-
@@ -96,92 +95,8 @@ constexpr int kGateTokens = 32;   // tokens per CTA iteration (2 groups of 16)
 constexpr int kGateKQ = 4;        // K split: warps (w >> 1) own H/4 columns each
 constexpr int kGateBatch = 8;     // 32-column steps whose loads are in flight together
 
-__global__ void __launch_bounds__(256) gate_logits_mma_kernel(const __nv_bfloat16* __restrict__ x,
-                                                              const float* __restrict__ w,
-                                                              const float* __restrict__ bias,
-                                                              float* __restrict__ logits, int T, int H, int E) {
-  extern __shared__ uint4 s_planes[];  // [3 planes][H/32 steps][32 lanes] : 8 bf16 each
-  __shared__ float s_red[2][kGateKQ][16][8];
-  const int n_steps = H / 32;
-  fill_gate_planes(s_planes, w, H, E);
-  __syncthreads();
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tg = warp & 1, kq = warp >> 1;
-  const int g = lane >> 2, t = lane & 3;
-  const int q_steps = n_steps / kGateKQ;  // steps owned by this warp (H % 128 == 0)
-  const int step0 = kq * q_steps;
-
-  for (int blk = blockIdx.x; blk * kGateTokens < T; blk += gridDim.x) {
-    const int row0 = blk * kGateTokens + tg * 16;
-    const int ra = min(row0 + g, T - 1), rb = min(row0 + g + 8, T - 1);
-    const __nv_bfloat16* pa = x + (size_t)ra * H + (size_t)step0 * 32 + t * 8;
-    const __nv_bfloat16* pb = x + (size_t)rb * H + (size_t)step0 * 32 + t * 8;
-    float c[4] = {0.f, 0.f, 0.f, 0.f};
-    for (int s0 = 0; s0 < q_steps; s0 += kGateBatch) {
-      uint4 va[kGateBatch], vb[kGateBatch];
-#pragma unroll
-      for (int b = 0; b < kGateBatch; ++b) {
-        if (s0 + b < q_steps) {
-          va[b] = ld_stream_16(pa + (s0 + b) * 32);
-          vb[b] = ld_stream_16(pb + (s0 + b) * 32);
-        }
-      }
-#pragma unroll
-      for (int b = 0; b < kGateBatch; ++b) {
-        if (s0 + b < q_steps) {
-          const int step = step0 + s0 + b;
-#pragma unroll
-          for (int p = 2; p >= 0; --p) {  // smallest plane first
-            const uint4 wf = s_planes[(p * n_steps + step) * 32 + lane];
-            mma_bf16_16x8x16(c, va[b].x, vb[b].x, va[b].y, vb[b].y, wf.x, wf.y);
-            mma_bf16_16x8x16(c, va[b].z, vb[b].z, va[b].w, vb[b].w, wf.z, wf.w);
-          }
-        }
-      }
-    }
-    // ---- reduce the K quarters; c0,c1 = (token g, experts 2t,2t+1), c2,c3 = (token g+8, same) -------------
-    s_red[tg][kq][g][2 * t] = c[0];
-    s_red[tg][kq][g][2 * t + 1] = c[1];
-    s_red[tg][kq][g + 8][2 * t] = c[2];
-    s_red[tg][kq][g + 8][2 * t + 1] = c[3];
-    __syncthreads();
-    if (kq == 0) {
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        const int r = g + 8 * half;
-        const int token = row0 + r;
-#pragma unroll
-        for (int z = 0; z < 2; ++z) {
-          const int e = 2 * t + z;
-          float s = s_red[tg][0][r][e];
-#pragma unroll
-          for (int q = 1; q < kGateKQ; ++q) s += s_red[tg][q][r][e];
-          if (token < T && e < E) logits[(size_t)token * E + e] = s + (bias ? bias[e] : 0.f);
-        }
-      }
-    }
-    __syncthreads();
-  }
-}
-
-int launch_gate_logits_mma(const __nv_bfloat16* x, const float* w, const float* bias, float* logits, int T, int H,
-                           int E, cudaStream_t st) {
-  const size_t smem = (size_t)3 * (H / 32) * 32 * sizeof(uint4);  // 48 * H bytes
-  if (E > 8 || H % 128 != 0 || smem > 200 * 1024) return -1;
-  static bool attr = false;
-  if (!attr) {
-    XTB_CUDA(cudaFuncSetAttribute(gate_logits_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
-  const int blocks = max(1, min(2 * sm_count(), (T + kGateTokens - 1) / kGateTokens));
-  gate_logits_mma_kernel<<<blocks, 256, smem, st>>>(x, w, bias, logits, T, H, E);
-  XTB_LAUNCH_OK();
-  return XTB_OK;
-}
-
 // ---- gate + greedy router + dispatch bucketing in ONE launch (xtb_gate_route_dispatch) -------------------------------
-// The tensor-core gate above already produces the logits of one 32-token block = one histogram chunk of the dispatch
+// The tensor-core gate produces the logits of one 32-token block = one histogram chunk of the dispatch
 // (dispatch_scan.cuh: kChunkTokens == 32) in shared memory; routing those 32 tokens there (one thread per token, E <= 8:
 // the same arithmetic, in the same order, as router_greedy_kernel<1, 8> in route.cu) and counting the chunk's expert
 // histogram with ballots removes the separate router launch (12.7 us per layer at C2, all latency) and the logits
@@ -283,7 +198,7 @@ __global__ void __launch_bounds__(256) gate_route_mma_kernel(
         if (s0 + b < q_steps) {
           const int step = step0 + s0 + b;
 #pragma unroll
-          for (int p = 2; p >= 0; --p) {
+          for (int p = 2; p >= 0; --p) {  // smallest plane first
             const uint4 wf = s_planes[(p * n_steps + step) * 32 + lane];
             mma_bf16_16x8x16(c, va[b].x, vb[b].x, va[b].y, vb[b].y, wf.x, wf.y);
             mma_bf16_16x8x16(c, va[b].z, vb[b].z, va[b].w, vb[b].w, wf.z, wf.w);
@@ -291,12 +206,13 @@ __global__ void __launch_bounds__(256) gate_route_mma_kernel(
         }
       }
     }
+    // ---- reduce the K quarters; c0,c1 = (token g, experts 2t,2t+1), c2,c3 = (token g+8, same) -------------
     s_red[tg][kq][g][2 * t] = c[0];
     s_red[tg][kq][g][2 * t + 1] = c[1];
     s_red[tg][kq][g + 8][2 * t] = c[2];
     s_red[tg][kq][g + 8][2 * t + 1] = c[3];
     __syncthreads();
-    {  // 256 threads = 32 tokens x 8 experts: same summation order over the K quarters as gate_logits_mma_kernel
+    {  // 256 threads = 32 tokens x 8 experts
       const int tok = threadIdx.x >> 3, e = threadIdx.x & 7;
       const int tgi = tok >> 4, r = tok & 15;
       float sacc = s_red[tgi][0][r][e];

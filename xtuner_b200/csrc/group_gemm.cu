@@ -13,8 +13,6 @@
 // SURVEY.md §8b "tokens_per_expert is a device tensor").  Ragged group boundaries: A tiles may over-read
 // into the next group's rows (masked at the store); for TN the partial last k-block is zero-filled in
 // shared memory before the MMA.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "sm100_ptx.cuh"
 
@@ -29,10 +27,8 @@ constexpr int kMaxExperts = 1024;
 constexpr int kGemmThreads = 384;
 constexpr int kConsumerWarps = 8;
 
-// STORE = 1 (default): every consumer warp packs 16-row x 64-column bf16 boxes into its own 2 KiB staging buffer (128-byte
-//            swizzle) and one lane issues a TMA store; boxes cut by a ragged expert boundary are copied out masked.
-// STORE = 0: registers -> 4-byte global stores.  Kept as the bit-identity yardstick of the default (XTB_GEMM_EPI=0;
-//            tests/test_gpu_group_gemm.py::test_tma_store_epilogue_is_bit_identical_to_direct_stores).
+// Epilogue: every consumer warp packs 16-row x 64-column bf16 boxes into its own 2 KiB staging buffer (128-byte swizzle)
+// and one lane issues a TMA store; boxes cut by a ragged expert boundary are copied out masked.
 template <int BLOCK_N>
 struct GemmCfg {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;  // 16 KiB
@@ -77,7 +73,7 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[BLOCK_N / 2], uint64_t da,
   else ptx::wgmma_m64n128k16_bf16<TA, TB>(d, da, db, accumulate);
 }
 
-template <int MODE, int BLOCK_N, int EPI, int STORE>
+template <int MODE, int BLOCK_N, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 group_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_o2,
@@ -109,15 +105,13 @@ group_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (lane == 0) {
       ptx::prefetch_tensormap(&tmap_a);
       ptx::prefetch_tensormap(&tmap_b);
-      if constexpr (STORE) {
-        ptx::prefetch_tensormap(&tmap_o);
-        if constexpr (EPI == EPI_SWIGLU) ptx::prefetch_tensormap(&tmap_o2);
-      }
+      ptx::prefetch_tensormap(&tmap_o);
+      if constexpr (EPI == EPI_SWIGLU) ptx::prefetch_tensormap(&tmap_o2);
       if constexpr (MODE == MODE_TN) {
         if (args.n_prob == 2) {
           ptx::prefetch_tensormap(&tmap_a2);
           ptx::prefetch_tensormap(&tmap_b2);
-          if constexpr (STORE) ptx::prefetch_tensormap(&tmap_o2);
+          ptx::prefetch_tensormap(&tmap_o2);
         }
       }
     }
@@ -259,44 +253,34 @@ group_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // rows [grow, grow+16) x columns [gcol, gcol+64) of the tensor behind `map`; `valid` = rows of this expert.
     auto emit_box = [&](const CUtensorMap* map, __nv_bfloat16* gbase, int ld, int gcol, int grow, int valid,
                         const uint32_t (&p0)[8], const uint32_t (&p1)[8]) {
-      if constexpr (STORE) {
-        if (lane == 0) ptx::bulk_wait_read_all();  // the previous store has finished reading the box
-        __syncwarp();
-        // 128-byte swizzle: 16-byte chunk j of row r lives at chunk j ^ (r & 7)
+      if (lane == 0) ptx::bulk_wait_read_all();  // the previous store has finished reading the box
+      __syncwarp();
+      // 128-byte swizzle: 16-byte chunk j of row r lives at chunk j ^ (r & 7)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t off = (uint32_t)r_lo * 128 + (uint32_t)((j ^ r_lo) << 4) + qc * 4;
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(box_u32 + off), "r"(p0[j]) : "memory");
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(box_u32 + off + 1024), "r"(p1[j]) : "memory");
-        }
-        ptx::fence_proxy_async_smem();
-        __syncwarp();
-        if (valid >= 16) {
-          if (lane == 0) {
-            ptx::tma_store_2d(map, box, gcol, grow);
-            ptx::bulk_commit_group();
-          }
-        } else {
-          // ragged boundary inside the box: masked copy of the valid rows, 8 lanes per 128-byte row
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int idx = i * 32 + lane;
-            const int r = idx >> 3, c = idx & 7;
-            if (r < valid) {
-              const uint4 v = *reinterpret_cast<const uint4*>(box + r * 128 + ((c ^ (r & 7)) << 4));
-              *reinterpret_cast<uint4*>(gbase + (size_t)(grow + r) * ld + gcol + c * 8) = v;
-            }
-          }
-          __syncwarp();
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t off = (uint32_t)r_lo * 128 + (uint32_t)((j ^ r_lo) << 4) + qc * 4;
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(box_u32 + off), "r"(p0[j]) : "memory");
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(box_u32 + off + 1024), "r"(p1[j]) : "memory");
+      }
+      ptx::fence_proxy_async_smem();
+      __syncwarp();
+      if (valid >= 16) {
+        if (lane == 0) {
+          ptx::tma_store_2d(map, box, gcol, grow);
+          ptx::bulk_commit_group();
         }
       } else {
-        uint32_t* d0 = reinterpret_cast<uint32_t*>(gbase + (size_t)(grow + r_lo) * ld + gcol + qc * 2);
-        uint32_t* d1 = reinterpret_cast<uint32_t*>(gbase + (size_t)(grow + r_lo + 8) * ld + gcol + qc * 2);
+        // ragged boundary inside the box: masked copy of the valid rows, 8 lanes per 128-byte row
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (r_lo < valid) d0[j * 4] = p0[j];
-          if (r_lo + 8 < valid) d1[j * 4] = p1[j];
+        for (int i = 0; i < 4; ++i) {
+          const int idx = i * 32 + lane;
+          const int r = idx >> 3, c = idx & 7;
+          if (r < valid) {
+            const uint4 v = *reinterpret_cast<const uint4*>(box + r * 128 + ((c ^ (r & 7)) << 4));
+            *reinterpret_cast<uint4*>(gbase + (size_t)(grow + r) * ld + gcol + c * 8) = v;
+          }
         }
+        __syncwarp();
       }
     };
 
@@ -453,9 +437,7 @@ group_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
       }
     }
-    if constexpr (STORE) {
-      if (lane == 0) ptx::bulk_wait_all();  // stores performed before the CTA exits
-    }
+    if (lane == 0) ptx::bulk_wait_all();  // stores performed before the CTA exits
   }
 }
 
@@ -485,49 +467,34 @@ static int make_tmap(CUtensorMap* map, const void* base, uint64_t rows, uint64_t
   return XTB_OK;
 }
 
-// XTB_GEMM_EPI=0 selects the direct-store epilogue (the bit-identity yardstick); default = TMA-store epilogue
-static bool gemm_epi_store() {
-  static const bool v = !(getenv("XTB_GEMM_EPI") && atoi(getenv("XTB_GEMM_EPI")) == 0);
-  return v;
-}
-
-template <int MODE, int BLOCK_N, int EPI, int STORE>
-static int launch_gemm_impl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const CUtensorMap& to2,
-                            const CUtensorMap& ta2, const CUtensorMap& tb2, const GemmArgs& args, cudaStream_t st) {
-  using Cfg = GemmCfg<BLOCK_N>;
-  static bool attr_set = false;
-  auto kfn = group_gemm_kernel<MODE, BLOCK_N, EPI, STORE>;
-  if (!attr_set) {
-    XTB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  XTB_CUDA(launch_pdl(kfn, dim3(sm_count()), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, st, ta, tb, to, to2, ta2, tb2, args));
-  XTB_LAUNCH_OK();
-  return XTB_OK;
-}
-
 // rows_out = rows of the 2-D view of `out` (and of `out2`, the SwiGLU epilogue's a[M, I]).  ta2 / tb2 / rows_out_b: the
 // operands and output rows of the second product of a two-product TN launch (args.n_prob == 2), else unused.
 template <int MODE, int BLOCK_N, int EPI = EPI_PLAIN>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& args, uint64_t rows_out,
                        cudaStream_t st, const CUtensorMap* ta2 = nullptr, const CUtensorMap* tb2 = nullptr,
                        uint64_t rows_out_b = 0) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  CUtensorMap to, to2;
+  int rc;
+  if ((rc = make_tmap(&to, args.out, rows_out, (uint64_t)args.ld_out, 16, 64))) return rc;
+  if constexpr (EPI == EPI_SWIGLU) {
+    if ((rc = make_tmap(&to2, args.out2, rows_out, (uint64_t)args.inter, 16, 64))) return rc;
+  } else if (MODE == MODE_TN && args.n_prob == 2) {
+    if ((rc = make_tmap(&to2, args.out_b, rows_out_b, (uint64_t)args.ld_out_b, 16, 64))) return rc;
+  } else {
+    to2 = to;
+  }
   const CUtensorMap& a2 = ta2 ? *ta2 : ta;
   const CUtensorMap& b2 = tb2 ? *tb2 : tb;
-  if (gemm_epi_store()) {
-    CUtensorMap to, to2;
-    int rc;
-    if ((rc = make_tmap(&to, args.out, rows_out, (uint64_t)args.ld_out, 16, 64))) return rc;
-    if constexpr (EPI == EPI_SWIGLU) {
-      if ((rc = make_tmap(&to2, args.out2, rows_out, (uint64_t)args.inter, 16, 64))) return rc;
-    } else if (MODE == MODE_TN && args.n_prob == 2) {
-      if ((rc = make_tmap(&to2, args.out_b, rows_out_b, (uint64_t)args.ld_out_b, 16, 64))) return rc;
-    } else {
-      to2 = to;
-    }
-    return launch_gemm_impl<MODE, BLOCK_N, EPI, 1>(ta, tb, to, to2, a2, b2, args, st);
+  static bool attr_set = false;
+  auto kfn = group_gemm_kernel<MODE, BLOCK_N, EPI>;
+  if (!attr_set) {
+    XTB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    attr_set = true;
   }
-  return launch_gemm_impl<MODE, BLOCK_N, EPI, 0>(ta, tb, ta, ta, a2, b2, args, st);
+  XTB_CUDA(launch_pdl(kfn, dim3(sm_count()), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, st, ta, tb, to, to2, a2, b2, args));
+  XTB_LAUNCH_OK();
+  return XTB_OK;
 }
 
 static int check_common(const void* a, const void* b, const int64_t* tpe, void* out, int64_t M_total, int N, int Kd,

@@ -3,8 +3,6 @@
 
 #include <cstring>
 
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace xtb {
@@ -22,11 +20,6 @@ int fail(int code, const char* fmt, ...) {
   vsnprintf(error_buffer(), 512, fmt, ap);
   va_end(ap);
   return code;
-}
-
-bool pdl_enabled() {
-  static const bool on = !(getenv("XTB_PDL") && atoi(getenv("XTB_PDL")) == 0);  // default on
-  return on;
 }
 
 int sm_count() {

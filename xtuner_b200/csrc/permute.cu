@@ -11,8 +11,6 @@
 //   dest(f)        = expert_start[e] + counts[c][e] + |{ f' in chunk c, f' < f, id[f'] == e }|
 // which is exactly the position a stable sort by expert id assigns (reference: argsort(stable=True),
 // ops/moe/cuda/permute_unpermute.py:215).
-#include <cstdlib>
-
 #include "common.cuh"
 #include "dispatch_scan.cuh"
 
@@ -48,8 +46,8 @@ __global__ void __launch_bounds__(256) permute_count_scan_kernel(const int32_t* 
 }
 
 // ---- kernel B: per-chunk stable ranks -> maps, then the row gather/scatter ---------------------------
-// One block per chunk.  COPY=false: index work only.
-template <bool COPY>
+// One block per sub-chunk.  The rows pass through registers: the path for rows too long to stage kSubTokens of in shared
+// memory (kernel B' below).
 __global__ void __launch_bounds__(128) permute_scatter_kernel(const uint4* __restrict__ x,
                                                               const int32_t* __restrict__ ids, int T, int K, int E,
                                                               int row_vec /* 16-byte vectors per row */,
@@ -83,7 +81,6 @@ __global__ void __launch_bounds__(128) permute_scatter_kernel(const uint4* __res
     row_id_map[fc + base + j] = dest;
     if (sorted_indices && dest >= 0) sorted_indices[dest] = fc + base + j;
   }
-  if (!COPY) return;
   __syncthreads();
 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
@@ -457,18 +454,16 @@ extern "C" size_t xtb_moe_permute_workspace_bytes(int T, int K, int E) {
 
 static int permute_impl(const void* x, const int32_t* ids, int T, int K, int E, int64_t row_bytes, void* permuted,
                         int32_t* row_id_map, int64_t* sorted_indices, int64_t* tokens_per_expert, void* workspace,
-                        xtb_stream_t stream, bool copy, bool prepared = false) {
+                        xtb_stream_t stream, bool prepared) {
   XTB_CHECK_ARG(ids && row_id_map && workspace, "xtb_moe_permute: null pointer");
   XTB_CHECK_ARG(T >= 0 && K > 0 && K <= 64 && E > 0 && E <= 1024, "xtb_moe_permute: bad T=%d K=%d E=%d", T, K, E);
   XTB_CHECK_ARG((int64_t)T * K < (1ll << 31), "xtb_moe_permute: T*K overflows int32");
   XTB_ENSURE_CTX(ids);
-  if (copy) {
-    XTB_CHECK_ARG(x && permuted, "xtb_moe_permute: null activation pointer");
-    XTB_CHECK_ARG(row_bytes > 0 && row_bytes % 16 == 0, "xtb_moe_permute: row_bytes=%lld must be a multiple of 16",
-                  (long long)row_bytes);
-    XTB_CHECK_ARG((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(permuted)) % 16 == 0,
-                  "xtb_moe_permute: pointers must be 16-byte aligned");
-  }
+  XTB_CHECK_ARG(x && permuted, "xtb_moe_permute: null activation pointer");
+  XTB_CHECK_ARG(row_bytes > 0 && row_bytes % 16 == 0, "xtb_moe_permute: row_bytes=%lld must be a multiple of 16",
+                (long long)row_bytes);
+  XTB_CHECK_ARG((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(permuted)) % 16 == 0,
+                "xtb_moe_permute: pointers must be 16-byte aligned");
   cudaStream_t st = as_stream(stream);
   if (T == 0) {
     if (tokens_per_expert) XTB_CUDA(cudaMemsetAsync(tokens_per_expert, 0, sizeof(int64_t) * E, st));
@@ -489,11 +484,10 @@ static int permute_impl(const void* x, const int32_t* ids, int T, int K, int E, 
     const size_t smem = (size_t)(kChunkTokens + kSubTokens) * K * sizeof(int);
     const int n_sub = (T + kSubTokens - 1) / kSubTokens;
     const int row_vec = (int)(row_bytes / 16);
-    // rows through shared memory with the bulk-copy engine (default; not compared with the register-staged kernel on
-    // H100).  XTB_PERMUTE_BULK=0 or rows too long for 8 staged rows: the register-staged kernel.
-    static const bool bulk = !(getenv("XTB_PERMUTE_BULK") && atoi(getenv("XTB_PERMUTE_BULK")) == 0);
+    // rows through shared memory with the bulk-copy engine; rows too long for kSubTokens staged rows (bf16 at K = 2:
+    // H >= 12784) through registers
     const size_t smem_bulk = (size_t)kSubTokens * row_bytes + kSubTokens * sizeof(uint64_t) + smem;
-    if (copy && bulk && smem_bulk <= 200 * 1024) {
+    if (smem_bulk <= 200 * 1024) {
       static bool attr = false;
       if (!attr) {
         XTB_CUDA(cudaFuncSetAttribute(permute_scatter_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -502,14 +496,12 @@ static int permute_impl(const void* x, const int32_t* ids, int T, int K, int E, 
       XTB_CUDA(launch_pdl(permute_scatter_bulk_kernel, dim3(n_sub), dim3(128), smem_bulk, st, static_cast<const uint8_t*>(x), ids, T, K, E, (uint32_t)row_bytes,
                                                                   w.counts, w.expert_start, static_cast<uint8_t*>(permuted),
                                                                   row_id_map, sorted_indices));
-    } else if (copy)
-      XTB_CUDA(launch_pdl(permute_scatter_kernel<true>, dim3(n_sub), dim3(128), smem, st, static_cast<const uint4*>(x), ids, T, K, E, row_vec,
+    } else {
+      XTB_CUDA(launch_pdl(permute_scatter_kernel, dim3(n_sub), dim3(128), smem, st, static_cast<const uint4*>(x), ids, T, K, E, row_vec,
                                                                 w.counts, w.expert_start,
                                                                 static_cast<uint4*>(permuted), row_id_map,
                                                                 sorted_indices));
-    else
-      XTB_CUDA(launch_pdl(permute_scatter_kernel<false>, dim3(n_sub), dim3(128), smem, st, nullptr, ids, T, K, E, 0, w.counts, w.expert_start,
-                                                                 nullptr, row_id_map, sorted_indices));
+    }
     XTB_LAUNCH_OK();
   }
   return XTB_OK;
@@ -519,21 +511,14 @@ extern "C" int xtb_moe_permute(const void* x, const int32_t* ids, int T, int K, 
                                void* permuted, int32_t* row_id_map, int64_t* sorted_indices,
                                int64_t* tokens_per_expert, void* workspace, xtb_stream_t stream) {
   return permute_impl(x, ids, T, K, E, row_bytes, permuted, row_id_map, sorted_indices, tokens_per_expert,
-                      workspace, stream, true);
+                      workspace, stream, false);
 }
 
 extern "C" int xtb_moe_permute_prepared(const void* x, const int32_t* ids, int T, int K, int E, int64_t row_bytes,
                                         void* permuted, int32_t* row_id_map, int64_t* sorted_indices,
                                         const void* prepared_workspace, xtb_stream_t stream) {
   return permute_impl(x, ids, T, K, E, row_bytes, permuted, row_id_map, sorted_indices, nullptr,
-                      const_cast<void*>(prepared_workspace), stream, true, true);
-}
-
-extern "C" int xtb_moe_permute_index(const int32_t* ids, int T, int K, int E, int32_t* row_id_map,
-                                     int64_t* sorted_indices, int64_t* tokens_per_expert, void* workspace,
-                                     xtb_stream_t stream) {
-  return permute_impl(nullptr, ids, T, K, E, 0, nullptr, row_id_map, sorted_indices, tokens_per_expert, workspace,
-                      stream, false);
+                      const_cast<void*>(prepared_workspace), stream, true);
 }
 
 // xtb_moe_combine and xtb_moe_unpermute; `entry` names the one that was called in the refusal messages

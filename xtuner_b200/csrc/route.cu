@@ -1,17 +1,10 @@
 // Router kernels (SURVEY.md §8a rows a1, a2, a2'): gate logits, greedy softmax/top-k router, no-aux
 // (DeepSeek-V3 style) router, and their backward passes.  All fp32 CUDA-core math — these ops are
 // HBM/latency bound ([T,E] tensors), not tensor-core work.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "dispatch_scan.cuh"
 
 namespace xtb {
-
-// gate_mma.cu: tensor-core variant of a1 — inside xtb_gate_route_dispatch by default; standalone (XTB_GATE_V=2) it is the
-// yardstick of that entry's bit-equality test (returns -1 when the shape is outside its domain)
-int launch_gate_logits_mma(const __nv_bfloat16* x, const float* w, const float* bias, float* logits, int T, int H,
-                           int E, cudaStream_t st);
 
 // =====================================================================================================
 // a1  gate logits, small-E specialisation (E <= 16): one warp streams TW tokens at a time; lane owns an
@@ -835,11 +828,6 @@ extern "C" int xtb_gate_logits(const void* x_bf16, const float* w_f32, const flo
   cudaStream_t st = as_stream(stream);
   const auto* x = static_cast<const __nv_bfloat16*>(x_bf16);
   const size_t w_smem = (size_t)E * H * sizeof(float);
-  static const int gate_v = getenv("XTB_GATE_V") ? atoi(getenv("XTB_GATE_V")) : 1;  // 2 = tensor-core kernel (test yardstick)
-  if (gate_v == 2) {
-    const int rc = launch_gate_logits_mma(x, w_f32, bias_f32, logits, T, H, E, st);
-    if (rc >= 0) return rc;  // -1: shape outside that kernel's domain, fall through
-  }
   if (E <= 16 && H % 256 == 0 && w_smem <= 200 * 1024) {
     const int blocks = min(sm_count(), (T + 63) / 64);
     if (E <= 8) {

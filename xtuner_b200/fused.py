@@ -14,7 +14,6 @@ launch-bound in eager mode otherwise.  Numerics are identical to composing
 """
 from __future__ import annotations
 
-import os
 from typing import Optional
 
 import torch
@@ -23,14 +22,6 @@ from torch import Tensor, nn
 from . import _capi, ops
 from ._capi import check, current_stream, ptr
 from .router import SCORING
-
-# ---- fused entry points (their A/B against the separate calls has not been repeated on H100); the env variables only exist so the
-# parity tests can still compare each fused kernel with the separate calls it replaces -----------------------------------
-# xtb_gate_route_dispatch : gate (tensor cores) + greedy router + dispatch bucketing in one launch (E <= 8, H % 128 == 0,
-#                           H <= 4096)
-# xtb_router_gate_bwd     : router backward in the prologue of the gate backward (E <= 8)
-GATE_ROUTE_FUSED = os.environ.get("XTB_GATE_ROUTE_FUSED", "1") == "1"
-ROUTER_GATE_BWD_FUSED = os.environ.get("XTB_ROUTER_GATE_BWD_FUSED", "1") == "1"
 
 # Where the next expert-weight gradients are written: a callable returning ``(g_w13_buffer, g_w2_buffer)`` (bf16, same
 # numel as the weights) or None.  The FSDP engine (fsdp_experts.py) points this at its symmetric gradient buffers so the
@@ -48,19 +39,38 @@ def _weight_grad_buffers(w13: Tensor, w2: Tensor):
     return torch.empty_like(w13), torch.empty_like(w2)
 
 
-def _gate_route_ok(H: int, E: int, K: int) -> bool:
-    return GATE_ROUTE_FUSED and E <= 8 and K <= 8 and H % 128 == 0 and H <= 4096
+def _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm, scaling, st):
+    """(logits, rw, tw, ids, ids32, tpe, ws): gate, greedy router and dispatch bucketing into the permute workspace ``ws``.
+    One launch (xtb_gate_route_dispatch: gate on the tensor cores) where E <= 8, K <= 8, H % 128 == 0 and H <= 4096, the
+    gate and the router as two calls otherwise (their A/B at the shapes both take has not been repeated on H100)."""
+    dev = x.device
+    logits = torch.empty((T, E), dtype=torch.float32, device=dev)
+    rw = torch.empty((T, E), dtype=torch.float32, device=dev)
+    tw = torch.empty((T, K), dtype=torch.float32, device=dev)
+    ids = torch.empty((T, K), dtype=torch.int64, device=dev)
+    ids32 = torch.empty((T, K), dtype=torch.int32, device=dev)
+    tpe = torch.empty((E,), dtype=torch.int64, device=dev)
+    ws = ops.permute_workspace(T, K, E, dev)
+    if E <= 8 and K <= 8 and H % 128 == 0 and H <= 4096:
+        _k(lib, "xtb_gate_route_dispatch", ptr(x), ptr(gate_w), T, H, E, K, scoring, int(norm), float(scaling),
+           ptr(logits), ptr(rw), ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
+    else:
+        _k(lib, "xtb_gate_logits", ptr(x), ptr(gate_w), None, ptr(logits), T, H, E, st)
+        _k(lib, "xtb_router_greedy_dispatch", ptr(logits), T, E, K, scoring, int(norm), float(scaling), ptr(rw), ptr(tw),
+           ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
+    return logits, rw, tw, ids, ids32, tpe, ws
 
 
 def _router_gate_bwd(lib, rw, tw, ids, g_tw, g_rw, g_lg, x, gate_w, T, H, E, K, scoring, norm, scaling, st):
-    """(grad_gate_w, grad_x_gate): router backward followed by the gate backward (one or two launches)."""
+    """(grad_gate_w, grad_x_gate): router backward followed by the gate backward, in one launch (xtb_router_gate_bwd: the
+    router backward in the prologue of the gate backward) where E <= 8 and H % 8 == 0, in two otherwise."""
     dev = x.device
     g_gate_w = torch.empty_like(gate_w)
     g_x_gate = torch.empty((T, H), dtype=torch.bfloat16, device=dev)
     wsb = ops._scratch("gate_bwd", int(lib.xtb_gate_logits_bwd_workspace_bytes(T, H, E)), dev)
     g_rw_c = None if g_rw is None else g_rw.contiguous()
     g_lg_c = None if g_lg is None else g_lg.contiguous()
-    if ROUTER_GATE_BWD_FUSED and E <= 8 and H % 8 == 0:
+    if E <= 8 and H % 8 == 0:
         _k(lib, "xtb_router_gate_bwd", ptr(rw), ptr(tw), ptr(ids), ptr(g_tw), ptr(g_rw_c), ptr(g_lg_c), ptr(x), ptr(gate_w),
            ptr(g_gate_w), ptr(g_x_gate), T, H, E, K, scoring, int(norm), float(scaling), ptr(wsb), st)
         return g_gate_w, g_x_gate
@@ -99,22 +109,9 @@ class FusedMoEFunction(torch.autograd.Function):
         K = top_k
         M = T * K
         dev = x.device
-        f32, bf = torch.float32, torch.bfloat16
+        bf = torch.bfloat16
 
-        logits = torch.empty((T, E), dtype=f32, device=dev)
-        rw = torch.empty((T, E), dtype=f32, device=dev)
-        tw = torch.empty((T, K), dtype=f32, device=dev)
-        ids = torch.empty((T, K), dtype=torch.int64, device=dev)
-        ids32 = torch.empty((T, K), dtype=torch.int32, device=dev)
-        tpe = torch.empty((E,), dtype=torch.int64, device=dev)
-        ws = ops.permute_workspace(T, K, E, dev)
-        if _gate_route_ok(H, E, K):
-            _k(lib, "xtb_gate_route_dispatch", ptr(x), ptr(gate_w), T, H, E, K, scoring, int(norm_topk_prob), float(scaling),
-               ptr(logits), ptr(rw), ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
-        else:
-            _k(lib, "xtb_gate_logits", ptr(x), ptr(gate_w), None, ptr(logits), T, H, E, st)
-            _k(lib, "xtb_router_greedy_dispatch", ptr(logits), T, E, K, scoring, int(norm_topk_prob), float(scaling), ptr(rw),
-               ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
+        logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st)
 
         x_perm = torch.empty((M, H), dtype=bf, device=dev)
         row_id_map = torch.empty((M,), dtype=torch.int32, device=dev)
@@ -197,24 +194,10 @@ class FusedMoEBlockFunction(torch.autograd.Function):
 
         x = torch.empty((T, H), dtype=bf, device=dev)
         rstd = torch.empty((T,), dtype=f32, device=dev)
-        logits = torch.empty((T, E), dtype=f32, device=dev)
         # the norm as its own streaming kernel: folding the gate into it (xtb_rmsnorm_gate with gate_w) is not used by
         # the fused layer (not measured on H100)
-        route_fused = _gate_route_ok(H, E, K)
         _k(lib, "xtb_rmsnorm_gate", ptr(h), ptr(norm_w), None, float(eps), T, H, E, ptr(x), ptr(rstd), None, st)
-        rw = torch.empty((T, E), dtype=f32, device=dev)
-        tw = torch.empty((T, K), dtype=f32, device=dev)
-        ids = torch.empty((T, K), dtype=torch.int64, device=dev)
-        ids32 = torch.empty((T, K), dtype=torch.int32, device=dev)
-        tpe = torch.empty((E,), dtype=torch.int64, device=dev)
-        ws = ops.permute_workspace(T, K, E, dev)
-        if route_fused:
-            _k(lib, "xtb_gate_route_dispatch", ptr(x), ptr(gate_w), T, H, E, K, scoring, int(norm_topk_prob), float(scaling),
-               ptr(logits), ptr(rw), ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
-        else:
-            _k(lib, "xtb_gate_logits", ptr(x), ptr(gate_w), None, ptr(logits), T, H, E, st)
-            _k(lib, "xtb_router_greedy_dispatch", ptr(logits), T, E, K, scoring, int(norm_topk_prob), float(scaling), ptr(rw),
-               ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
+        logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st)
         x_perm = torch.empty((M, H), dtype=bf, device=dev)
         row_id_map = torch.empty((M,), dtype=torch.int32, device=dev)
         _k(lib, "xtb_moe_permute_prepared", ptr(x), ptr(ids32), T, K, E, H * 2, ptr(x_perm), ptr(row_id_map), None, ptr(ws), st)
