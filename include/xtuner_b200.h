@@ -249,6 +249,37 @@ int xtb_moe_dispatch_bwd_rmsnorm(const void* g_xperm_bf16, const int32_t* row_id
                                  const void* g_res_bf16, int T, int K, int H, void* g_h_bf16, float* g_norm_w,
                                  void* workspace, xtb_stream_t stream);
 
+/* q_norm / k_norm and the rotary embedding in front of the attention (MultiHeadAttention.forward,
+ * module/attention/mha.py:353-363: RMSNorm = F.rms_norm, ops/rms_norm/__init__.py:8-11, then
+ * apply_rotary_pos_emb_cuda, ops/rotary_emb.py:18-49), one kernel each way for q and k together.
+ *   q [T, Hq, D], k [T, Hkv, D] bf16 with any token / head stride (elements, multiples of 8) and the D axis contiguous;
+ *   cos, sin [T, D] bf16 contiguous (all D columns are read); w_q, w_k [D] fp32, or both NULL for qk_norm=False.
+ *   half = D/2, D in {64, 128, 256} (XTB_ERR_INVALID otherwise); pointers 16-byte aligned.
+ * Forward, per (token, head) row x:
+ *   rstd  = rsqrtf(mean(x^2) + eps) in fp32, written to rstd_q [T, Hq] / rstd_k [T, Hkv]   (norm only)
+ *   n_i   = bf16((x_i rstd) w_i)                 (n = x without the norm)
+ *   r_i   = -n_{i+half} for i < half, n_{i-half} otherwise                        (rotate_half)
+ *   out_i = bf16( bf16(n_i cos_i) + bf16(r_i sin_i) )  into contiguous out_q [T, Hq, D], out_k [T, Hkv, D]
+ * Backward, g = grad of out (same stride rules as q / k):
+ *   gn_i  = bf16( bf16(g_i cos_i) + bf16(g_{i+half} sin_{i+half}) )   for i < half
+ *   gn_i  = bf16( bf16(g_i cos_i) - bf16(g_{i-half} sin_{i-half}) )   for i >= half   (autograd's roundings)
+ *   dx    = bf16( (w gn - x c) rstd ),  c = (sum_i w_i gn_i x_i) rstd^2 / D           (dx = gn without the norm)
+ *   dw    [2D] fp32 = [dw_q | dw_k], dw_q = sum over (t, h) of gn x rstd, summed in a fixed order (identical bits run to
+ *         run); NULL to skip, needs xtb_qk_norm_rope_bwd_workspace_bytes(T, D) bytes of workspace.  cos and sin get no
+ *         gradient.  dx_q / dx_k are contiguous [T, Hq, D] / [T, Hkv, D].
+ * T = 0 is a no-op (the backward then writes dw = 0).  Byte offsets are 64-bit: T * H * D may exceed 2^31. */
+int xtb_qk_norm_rope(const void* q_bf16, int64_t q_stride_t, int64_t q_stride_h, const void* k_bf16, int64_t k_stride_t,
+                     int64_t k_stride_h, const void* cos_bf16, const void* sin_bf16, const float* w_q_f32,
+                     const float* w_k_f32, float eps, int T, int Hq, int Hkv, int D, void* out_q_bf16, void* out_k_bf16,
+                     float* rstd_q, float* rstd_k, xtb_stream_t stream);
+size_t xtb_qk_norm_rope_bwd_workspace_bytes(int T, int D);
+int xtb_qk_norm_rope_bwd(const void* g_q_bf16, int64_t g_q_stride_t, int64_t g_q_stride_h, const void* g_k_bf16,
+                         int64_t g_k_stride_t, int64_t g_k_stride_h, const void* q_bf16, int64_t q_stride_t,
+                         int64_t q_stride_h, const void* k_bf16, int64_t k_stride_t, int64_t k_stride_h,
+                         const void* cos_bf16, const void* sin_bf16, const float* w_q_f32, const float* w_k_f32,
+                         const float* rstd_q, const float* rstd_k, int T, int Hq, int Hkv, int D, void* dx_q_bf16,
+                         void* dx_k_bf16, float* dw, void* workspace, xtb_stream_t stream);
+
 /* ==== fp8 tile-wise quantisation (row a15, config 5) ============================================================
  * e4m3, scale = clamp(amax, 1e-12) / 448 (xtuner/v1/float8/float8_utils.py:6-32, fsdp_utils.py:75-116,195-223,
  * triton_kernels/per_tile_quant.py:61-100).  Bit-exact against reference-made golden vectors on an H100

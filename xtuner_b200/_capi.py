@@ -92,6 +92,18 @@ SIGNATURES = {
         [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
          c_void_p, c_void_p],
     ),
+    "xtb_qk_norm_rope": (
+        c_int,
+        [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int,
+         c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
+    "xtb_qk_norm_rope_bwd_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "xtb_qk_norm_rope_bwd": (
+        c_int,
+        [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64,
+         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+         c_void_p, c_void_p],
+    ),
     "xtb_fp8_per_tile_quant": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "xtb_fp8_block_scales": (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_void_p, c_void_p]),
     "xtb_fp8_block_cast": (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),

@@ -20,7 +20,8 @@ from torch import Tensor
 from . import _capi
 from ._capi import check, current_stream, ptr
 
-__all__ = ["permute", "unpermute", "group_gemm", "swiglu", "gate_logits", "permute_workspace", "lm_head_cross_entropy"]
+__all__ = ["permute", "unpermute", "group_gemm", "swiglu", "gate_logits", "permute_workspace", "lm_head_cross_entropy",
+           "qk_norm_rope"]
 
 
 def _require_cuda(*tensors: Tensor) -> None:
@@ -520,6 +521,143 @@ def lm_head_cross_entropy(hidden: Tensor, weight: Tensor, labels: Tensor, loss_w
         raise ValueError(f"lm_head_cross_entropy: chunk_size must be positive (got {chunk_size})")
     need_grad = torch.is_grad_enabled() and (hidden.requires_grad or weight.requires_grad)
     return _LMHeadCrossEntropy.apply(h, weight.contiguous(), lab, lw, int(ignore_index), chunk_size, need_grad)
+
+
+# ======================================================================================================
+# q/k RMSNorm + rotary embedding in front of the attention (MultiHeadAttention.forward, mha.py:353-363)
+# ======================================================================================================
+
+
+def _rows(t: Tensor) -> Tuple[int, int]:
+    """(token stride, head stride) in elements of a [T, H, D] operand"""
+    return t.stride(0), t.stride(1)
+
+
+@torch.library.custom_op("xtuner_b200::qk_norm_rope", mutates_args=())
+def _qk_norm_rope_op(q: Tensor, k: Tensor, cos: Tensor, sin: Tensor, w_q: Optional[Tensor], w_k: Optional[Tensor],
+                     eps: float) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+    """-> (out_q [T, Hq, D], out_k [T, Hkv, D], rstd_q fp32 [T, Hq], rstd_k fp32 [T, Hkv]); the rstd are empty without a
+    norm weight"""
+    lib = _capi.ensure_init()
+    q, k = _strided_rows(q), _strided_rows(k)
+    T, Hq, D = q.shape
+    Hkv = k.shape[1]
+    out_q, out_k = q.new_empty((T, Hq, D)), k.new_empty((T, Hkv, D))
+    norm = w_q is not None
+    rstd_q = q.new_empty((T, Hq) if norm else (0,), dtype=torch.float32)
+    rstd_k = k.new_empty((T, Hkv) if norm else (0,), dtype=torch.float32)
+    if T == 0:
+        return out_q, out_k, rstd_q, rstd_k
+    check(
+        lib.xtb_qk_norm_rope(
+            ptr(q), *_rows(q), ptr(k), *_rows(k), ptr(cos), ptr(sin), ptr(w_q), ptr(w_k), eps, T, Hq, Hkv, D, ptr(out_q),
+            ptr(out_k), ptr(rstd_q) if norm else None, ptr(rstd_k) if norm else None, current_stream(),
+        ),
+        "xtb_qk_norm_rope",
+    )
+    return out_q, out_k, rstd_q, rstd_k
+
+
+@_qk_norm_rope_op.register_fake
+def _(q, k, cos, sin, w_q, w_k, eps):
+    norm = w_q is not None
+    return (q.new_empty(q.shape), k.new_empty(k.shape),
+            q.new_empty(q.shape[:2] if norm else (0,), dtype=torch.float32),
+            k.new_empty(k.shape[:2] if norm else (0,), dtype=torch.float32))
+
+
+@torch.library.custom_op("xtuner_b200::qk_norm_rope_bwd", mutates_args=())
+def _qk_norm_rope_bwd_op(g_q: Tensor, g_k: Tensor, q: Tensor, k: Tensor, cos: Tensor, sin: Tensor, w_q: Optional[Tensor],
+                         w_k: Optional[Tensor], rstd_q: Tensor, rstd_k: Tensor, need_dw: bool
+                         ) -> Tuple[Tensor, Tensor, Tensor]:
+    """-> (dx_q [T, Hq, D], dx_k [T, Hkv, D], dw fp32 [2, D] = (dw_q, dw_k), empty unless ``need_dw``)"""
+    lib = _capi.ensure_init()
+    g_q, g_k, q, k = (_strided_rows(t) for t in (g_q, g_k, q, k))
+    T, Hq, D = q.shape
+    Hkv = k.shape[1]
+    dx_q, dx_k = q.new_empty((T, Hq, D)), k.new_empty((T, Hkv, D))
+    norm = w_q is not None
+    need_dw = need_dw and norm
+    dw = q.new_empty((2, D) if need_dw else (0,), dtype=torch.float32)
+    if T == 0:
+        return dx_q, dx_k, dw.zero_()
+    ws = _scratch("qk_norm_rope_bwd", int(lib.xtb_qk_norm_rope_bwd_workspace_bytes(T, D)), q.device) if need_dw else None
+    check(
+        lib.xtb_qk_norm_rope_bwd(
+            ptr(g_q), *_rows(g_q), ptr(g_k), *_rows(g_k), ptr(q), *_rows(q), ptr(k), *_rows(k), ptr(cos), ptr(sin), ptr(w_q),
+            ptr(w_k), ptr(rstd_q) if norm else None, ptr(rstd_k) if norm else None, T, Hq, Hkv, D, ptr(dx_q), ptr(dx_k),
+            ptr(dw) if need_dw else None, ptr(ws), current_stream(),
+        ),
+        "xtb_qk_norm_rope_bwd",
+    )
+    return dx_q, dx_k, dw
+
+
+@_qk_norm_rope_bwd_op.register_fake
+def _(g_q, g_k, q, k, cos, sin, w_q, w_k, rstd_q, rstd_k, need_dw):
+    need = need_dw and w_q is not None
+    return q.new_empty(q.shape), k.new_empty(k.shape), q.new_empty((2, q.shape[2]) if need else (0,), dtype=torch.float32)
+
+
+class _QKNormRope(torch.autograd.Function):
+    """q_norm / k_norm (``F.rms_norm``) followed by ``apply_rotary_pos_emb_cuda`` as one node.  Saves the projections
+    (which the reference keeps alive too), the two rstd, cos and sin; no normalised copy."""
+
+    @staticmethod
+    def forward(ctx, q: Tensor, k: Tensor, cos: Tensor, sin: Tensor, w_q: Optional[Tensor], w_k: Optional[Tensor],
+                eps: float):
+        out_q, out_k, rstd_q, rstd_k = _qk_norm_rope_op(q, k, cos, sin, w_q, w_k, eps)
+        ctx.save_for_backward(q, k, cos, sin, w_q, w_k, rstd_q, rstd_k)
+        ctx.mark_non_differentiable(rstd_q, rstd_k)
+        return out_q, out_k, rstd_q, rstd_k
+
+    @staticmethod
+    def backward(ctx, g_q, g_k, _g_rq, _g_rk):
+        q, k, cos, sin, w_q, w_k, rstd_q, rstd_k = ctx.saved_tensors
+        need_dw = w_q is not None and (ctx.needs_input_grad[4] or ctx.needs_input_grad[5])
+        g_q = torch.zeros_like(q) if g_q is None else g_q
+        g_k = torch.zeros_like(k) if g_k is None else g_k
+        dx_q, dx_k, dw = _qk_norm_rope_bwd_op(g_q, g_k, q, k, cos, sin, w_q, w_k, rstd_q, rstd_k, need_dw)
+        dw_q = dw[0] if need_dw and ctx.needs_input_grad[4] else None
+        dw_k = dw[1] if need_dw and ctx.needs_input_grad[5] else None
+        return dx_q, dx_k, None, None, dw_q, dw_k, None
+
+
+def _strided_rows(t: Tensor) -> Tensor:
+    """``t`` itself when the kernels can read it in place ([T, H, D] with the D axis contiguous and 16-byte aligned rows),
+    otherwise a contiguous copy.  Called inside the custom ops, which always see real tensors."""
+    if t.stride(2) == 1 and t.stride(0) % 8 == 0 and t.stride(1) % 8 == 0 and t.data_ptr() % 16 == 0:
+        return t
+    return t.contiguous()
+
+
+def qk_norm_rope(q: Tensor, k: Tensor, cos: Tensor, sin: Tensor, q_norm_weight: Tensor | None = None,
+                 k_norm_weight: Tensor | None = None, eps: float = 1e-6) -> Tuple[Tensor, Tensor]:
+    """``apply_rotary_pos_emb_cuda(q_norm(q), k_norm(k), cos, sin)`` of ``MultiHeadAttention`` (mha.py:353-363) with the
+    reference's roundings (``include/xtuner_b200.h``): ``q`` ``[T, Hq, D]`` and ``k`` ``[T, Hkv, D]`` bf16 (any token and
+    head strides; the D axis contiguous), ``cos``/``sin`` ``[T, D]`` bf16, norm weights ``[D]`` (fp32 or bf16) or both
+    None to skip the norm.  D is 64, 128 or 256.  Returns contiguous ``(q_embed [T, Hq, D], k_embed [T, Hkv, D])``; the
+    weight gradients come back in the weights' dtype."""
+    _require_cuda(q, k, cos, sin, q_norm_weight, k_norm_weight)
+    for t, name in ((q, "q"), (k, "k"), (cos, "cos"), (sin, "sin")):
+        _bf16(t, name)
+    if (q_norm_weight is None) != (k_norm_weight is None):
+        raise ValueError("qk_norm_rope: pass both norm weights or neither")
+    if q.dim() != 3 or k.dim() != 3 or k.shape[0] != q.shape[0] or k.shape[2] != q.shape[2]:
+        raise _capi.XtbError(f"qk_norm_rope: q must be [T, Hq, D] and k [T, Hkv, D] (got {tuple(q.shape)}, {tuple(k.shape)})")
+    T, _, D = q.shape
+    if D not in (64, 128, 256):
+        raise _capi.XtbError(f"qk_norm_rope: head dim {D} is not 64, 128 or 256")
+    cos, sin = cos.reshape(-1, cos.shape[-1]), sin.reshape(-1, sin.shape[-1])
+    if tuple(cos.shape) != (T, D) or tuple(sin.shape) != (T, D):
+        raise _capi.XtbError(f"qk_norm_rope: cos and sin must be [{T}, {D}] (got {tuple(cos.shape)}, {tuple(sin.shape)})")
+    w_q = w_k = None
+    if q_norm_weight is not None:
+        if tuple(q_norm_weight.shape) != (D,) or tuple(k_norm_weight.shape) != (D,):
+            raise _capi.XtbError(f"qk_norm_rope: norm weights must be [{D}]")
+        w_q, w_k = q_norm_weight.float().contiguous(), k_norm_weight.float().contiguous()  # bf16 widens exactly
+    out_q, out_k, _, _ = _QKNormRope.apply(q, k, cos.contiguous(), sin.contiguous(), w_q, w_k, float(eps))
+    return out_q, out_k
 
 
 # ======================================================================================================

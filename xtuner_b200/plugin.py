@@ -16,7 +16,8 @@ autograd node (:func:`xtuner_b200.fused.fused_moe_block`), the form ``bench.py``
 installed for the paths the fused node does not cover (micro-batched forward, rollout-routed experts).
 
 Everything else of the model (attention, norms, lm_head, FSDP wrapping, checkpoint keys) is untouched;
-``install_lm_head_loss()`` separately moves the lm_head cross-entropy onto this package's kernels; parameters keep
+``install_lm_head_loss()`` separately moves the lm_head cross-entropy onto this package's kernels, and
+``install_qk_norm_rope(model)`` the q/k norm and rotary embedding in front of the attention; parameters keep
 their names, so state dicts and DCP checkpoints stay compatible.  ``restore_model`` undoes the conversion.
 """
 from __future__ import annotations
@@ -351,3 +352,95 @@ def uninstall_fp8_cast() -> None:
     if hasattr(fu, _SAVED):
         fu.cast_to_per_block_fp8_with_scales, fu.tensor_to_per_block_fp8_scales = getattr(fu, _SAVED)
         delattr(fu, _SAVED)
+
+
+# ======================================================================================================
+# q/k RMSNorm + rotary embedding in front of the attention (SURVEY.md §8f-3)
+# ======================================================================================================
+
+_QK_SAVED = "_xtuner_b200_qk_saved"
+
+
+def _qk_layer_eligible(attn: nn.Module, apply_rotary_pos_emb_cuda) -> bool:
+    """what ``ops.qk_norm_rope`` computes: the full-width rotary embedding (not partial rotary or FoPE sep-head), the
+    "default" RMSNorm (or none), one eps for both norms, head dim 64, 128 or 256"""
+    if vars(attn).get("apply_rotary_emb") is not apply_rotary_pos_emb_cuda or attn.head_dim not in (64, 128, 256):
+        return False
+    if not attn.qk_norm:
+        return True
+    qn, kn = attn.q_norm, attn.k_norm
+    return (getattr(qn, "_type", None) == "default" and getattr(kn, "_type", None) == "default"
+            and qn.variance_epsilon == kn.variance_epsilon and "forward" not in vars(qn) and "forward" not in vars(kn))
+
+
+def _qk_call_eligible(q, k, cos, sin, position_ids, unsqueeze_dim) -> bool:
+    """[1, H, S, D] bf16 CUDA q / k with the D axis contiguous, [1, S, D] cos / sin"""
+    return (unsqueeze_dim == 1 and position_ids is None
+            and all(type(t) in (torch.Tensor, nn.Parameter) and _on_device(t) and t.dtype == torch.bfloat16
+                    for t in (q, k, cos, sin))
+            and q.dim() == 4 and k.dim() == 4 and q.shape[0] == 1 and k.shape[0] == 1 and q.stride(-1) == 1
+            and k.stride(-1) == 1 and cos.dim() == 3 and cos.shape[0] == 1 and sin.shape == cos.shape
+            and cos.shape[1] == q.shape[2] and cos.shape[2] == q.shape[3])
+
+
+def _qk_rope_closure(attn: nn.Module, orig_rope, norms):
+    """the ``ApplyRotaryEmbProtocol`` callable set on ``attn``: with the norms made pass-throughs, it receives the raw
+    projections and runs norm + rope as one op; calls it does not cover run the saved norm forwards and the original rope"""
+
+    def apply_rotary_emb(q, k, cos, sin, position_ids=None, unsqueeze_dim=1):
+        if not _qk_call_eligible(q, k, cos, sin, position_ids, unsqueeze_dim):
+            if norms is not None:  # RMSNorm over the last dim: the same values on the transposed view
+                q, k = norms[0](q), norms[1](k)
+            return orig_rope(q, k, cos, sin, position_ids, unsqueeze_dim)
+        w_q = w_k = None
+        eps = 1e-6
+        if norms is not None:
+            w_q, w_k = _local(attn.q_norm.weight), _local(attn.k_norm.weight)
+            eps = attn.q_norm.variance_epsilon
+        S, D = q.shape[2], q.shape[3]
+        out_q, out_k = ops.qk_norm_rope(q[0].transpose(0, 1), k[0].transpose(0, 1), cos[0], sin[0], w_q, w_k, eps)
+        return out_q.view(1, S, -1, D).transpose(1, 2), out_k.view(1, S, -1, D).transpose(1, 2)
+
+    apply_rotary_emb.__wrapped__ = orig_rope
+    return apply_rotary_emb
+
+
+def _identity(hidden_states):
+    return hidden_states
+
+
+def install_qk_norm_rope(model: nn.Module) -> int:
+    """Runs q_norm / k_norm and the rotary embedding of every eligible ``MultiHeadAttention``
+    (``xtuner/v1/module/attention/mha.py``) as one fused op (:func:`ops.qk_norm_rope`) in ``forward``, ``prefilling`` and
+    ``decoding``.  The seam is the reference's own per-instance ``apply_rotary_emb`` (set at ``mha.py:202``); with
+    ``qk_norm`` the two norms' ``forward`` become per-instance pass-throughs and the rope reads their weights at call time,
+    so module objects, parameters and state-dict keys stay as they are.  Layers with partial rotary, FoPE sep-head or the
+    zero-centred norm are left alone; calls outside [1, H, S, D] bf16 CUDA tensors run the original norms and rope.
+    Opt-in and separate from :func:`convert_model`.  Returns the number of attention modules changed."""
+    mha = importlib.import_module("xtuner.v1.module.attention.mha")
+    rope = importlib.import_module("xtuner.v1.ops.rotary_emb").apply_rotary_pos_emb_cuda
+    n = 0
+    for attn in model.modules():
+        if not isinstance(attn, mha.MultiHeadAttention) or _QK_SAVED in vars(attn) or not _qk_layer_eligible(attn, rope):
+            continue
+        orig = attn.apply_rotary_emb
+        norms = None
+        if attn.qk_norm:
+            norms = (attn.q_norm.forward, attn.k_norm.forward)
+            attn.q_norm.forward = _identity
+            attn.k_norm.forward = _identity
+        attn.apply_rotary_emb = _qk_rope_closure(attn, orig, norms)
+        setattr(attn, _QK_SAVED, orig)
+        n += 1
+    return n
+
+
+def uninstall_qk_norm_rope(model: nn.Module) -> None:
+    for attn in model.modules():
+        if _QK_SAVED not in vars(attn):
+            continue
+        attn.apply_rotary_emb = vars(attn)[_QK_SAVED]
+        if attn.qk_norm:
+            del attn.q_norm.forward
+            del attn.k_norm.forward
+        delattr(attn, _QK_SAVED)
