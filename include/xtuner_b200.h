@@ -81,10 +81,10 @@ int xtb_router_greedy_dispatch(const float* logits, int T, int E, int K, int sco
                                int32_t* topk_ids_i32, int64_t* tokens_per_expert, void* dispatch_workspace,
                                xtb_stream_t stream);
 /* a1 + a2 + the index half of a4 in ONE launch (csrc/gate_mma.cu) — what the fused layer calls.  Gate logits on the
- * tensor cores (fp32 weight as three bf16 planes, exact products, fp32 accumulation), then the greedy router of
- * xtb_router_greedy_dispatch on the 32-token block that is still in shared memory, then the chunk histograms and their
- * scan: the outputs of xtb_gate_logits (no bias) followed by xtb_router_greedy_dispatch, one kernel instead of two and
- * no logits round trip.  The logits equal float64 on exact inputs and stay within the bound of
+ * tensor cores (fp32 weight as three bf16 planes, exact products, fp32 accumulation), then the per-token code of
+ * xtb_router_greedy_dispatch itself (csrc/greedy_router.cuh) on the 32-token block that is still in shared memory, then
+ * the chunk histograms and their scan: the outputs of xtb_gate_logits (no bias) followed by xtb_router_greedy_dispatch,
+ * one kernel instead of two and no logits round trip.  The logits equal float64 on exact inputs and stay within the bound of
  * tests/router_reference.py otherwise; every other output, the dispatch workspace included, is bit-equal on an H100 to
  * xtb_router_greedy_dispatch run on those logits (tests/test_gpu_router_edges.py).  E <= 8, K <= 8, H % 128 == 0,
  * H <= 4224; XTB_ERR_INVALID otherwise (use the two calls). */
@@ -101,9 +101,9 @@ int xtb_router_greedy_bwd(const float* router_weights, const float* topk_weights
                           float scaling, float* grad_logits, xtb_stream_t stream);
 
 /* backward of a2 and of a1 in ONE launch — what the fused layer calls; bit-equal on an H100 to xtb_router_greedy_bwd +
- * xtb_gate_logits_bwd (tests/test_gpu_router_edges.py): grad_logits is computed per token in the
- * prologue of the gate backward (same formula and order as xtb_router_greedy_bwd) and never written to memory;
- * grad_w / grad_x as xtb_gate_logits_bwd (no bias).  workspace: xtb_gate_logits_bwd_workspace_bytes(T, H, E).
+ * xtb_gate_logits_bwd (tests/test_gpu_router_edges.py): grad_logits is computed per token in the prologue of the
+ * gate backward by the per-token code of xtb_router_greedy_bwd itself (csrc/greedy_router.cuh) and never written to
+ * memory; grad_w / grad_x as xtb_gate_logits_bwd (no bias).  workspace: xtb_gate_logits_bwd_workspace_bytes(T, H, E).
  * E <= 8, H % 8 == 0; XTB_ERR_INVALID otherwise (use the two calls). */
 int xtb_router_gate_bwd(const float* router_weights, const float* topk_weights, const int64_t* topk_ids,
                         const float* grad_topk_weights, const float* grad_router_weights,

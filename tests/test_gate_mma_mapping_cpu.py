@@ -94,8 +94,10 @@ def test_gate_mma_index_model(T, H, E):
     np.testing.assert_allclose(logits, ref, rtol=1e-6, atol=1e-6)
 
 
-def _route_token_e8(lg, E, K, scoring, norm_topk, scaling):
-    """``route_token_e8`` of csrc/gate_mma.cu, statement by statement (float32 arithmetic)."""
+def _greedy_route_token(lg, E, K, scoring, norm_topk, scaling):
+    """``greedy_route_token<1, 8>`` of csrc/greedy_router.cuh (the router of the one-launch gate+router kernel), statement
+    by statement (float32 arithmetic).  With one lane per token the group shuffles are empty and the kernel's two
+    selection masks, ``taken`` (this lane's experts) and ``used`` (the token's), are one."""
     f32 = np.float32
     p = np.full(8, -np.inf, f32)
     p[:E] = lg[:E]
@@ -109,16 +111,16 @@ def _route_token_e8(lg, E, K, scoring, norm_topk, scaling):
     else:
         for j in range(8):
             p[j] = f32(1) / (f32(1) + np.exp(-p[j], dtype=f32)) if j < E else -np.inf
-    taken, total = 0, f32(0)
+    used, total = 0, f32(0)
     wv, se = np.zeros(K, f32), np.zeros(K, np.int64)
     for k in range(K):
         bv, be = -np.inf, 0x7FFFFFFF
         for j in range(8):
-            if not (taken >> j) & 1 and j < E and p[j] > bv:
+            if not (used >> j) & 1 and j < E and p[j] > bv:
                 bv, be = p[j], j
-        if be < 0 or be >= E:
-            be, bv = k, f32(0)
-        taken |= 1 << be
+        if be < 0 or be >= E:  # NaN rows: the lowest index not selected yet
+            be, bv = next(e for e in range(E) if not (used >> e) & 1), f32(0)
+        used |= 1 << be
         wv[k], se[k] = bv, be
         total = f32(total + bv)
     for k in range(K):
@@ -143,7 +145,7 @@ def test_route_token_model_matches_oracle_router(E, K, scoring, norm, scaling):
     ids = np.zeros((T, K), np.int64)
     with np.errstate(over="ignore", invalid="ignore"):
         for t in range(T):
-            p, wv, se = _route_token_e8(np.pad(lg[t].numpy(), (0, 8 - E)), E, K, 0 if scoring == "softmax" else 1, norm, scaling)
+            p, wv, se = _greedy_route_token(np.pad(lg[t].numpy(), (0, 8 - E)), E, K, 0 if scoring == "softmax" else 1, norm, scaling)
             ids[t] = se
             np.testing.assert_allclose(p[:E], ref["router_weights"][t].numpy(), rtol=2e-6, atol=1e-7)
             np.testing.assert_allclose(wv, ref["topk_weights"][t].numpy(), rtol=2e-6, atol=1e-7)
@@ -157,3 +159,18 @@ def test_route_token_model_matches_oracle_router(E, K, scoring, norm, scaling):
                 ballot = [(c * 32 + lane < T) and ids[min(c * 32 + lane, T - 1), k] == e for lane in range(32)]
                 counts[c, e] += sum(ballot)
     assert np.array_equal(counts.sum(0), ref["topkens_per_expert"].numpy())
+
+
+def test_route_token_model_nan_fallback_after_a_gap():
+    """A row whose NaN experts run the top-k out of comparable scores after a gap in the selected ids: the fallback takes
+    the lowest id not selected yet (1), not the round number (2).  Written out by hand: torch.topk, and so the oracle,
+    ranks NaN first."""
+    f32 = np.float32
+    lg = np.array([3, np.nan, 2, np.nan, 0, 0, 0, 0], f32)
+    with np.errstate(invalid="ignore"):
+        p, wv, se = _greedy_route_token(lg, 4, 3, 1, True, 1.0)
+    s3, s2 = f32(1) / (f32(1) + np.exp(f32(-3))), f32(1) / (f32(1) + np.exp(f32(-2)))
+    assert se.tolist() == [0, 2, 1]
+    np.testing.assert_array_equal(p[[0, 2]], [s3, s2])
+    assert np.isnan(p[[1, 3]]).all()
+    np.testing.assert_array_equal(wv, [s3 / f32(s3 + s2), s2 / f32(s3 + s2), 0])

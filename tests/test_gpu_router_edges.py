@@ -11,9 +11,10 @@ of tests/router_reference.py, at the edges the parity tests of tests/test_gpu_ro
   bound, ids equal to float64 on decided rows.  Tie rows, rows of tied zeros, NaN and +-inf rows.  Refusals.
 * Fused gate + route + dispatch bit-equal to xtb_router_greedy_dispatch on its own logits, and the rows
   xtb_moe_permute_prepared gathers from either workspace bit-equal, at E = 1 to 8, K = 1 to E and at the benchmark
-  shape (T = 8192, H = 2048, E = 8, K = 2).
+  shape (T = 8192, H = 2048, E = 8, K = 2), and on logits with tie, NaN, partial-NaN and +-inf rows at E = 4 and 8.
 * Backward: xtb_router_greedy_bwd against float64 autograd with every null combination of the three gradients;
-  xtb_router_gate_bwd bit-equal to the two calls it replaces at E = 1 to 8, K = 1 to E and at the benchmark shape; the
+  xtb_router_gate_bwd bit-equal to the two calls it replaces at E = 1 to 8, K = 1 to E and at the benchmark shape,
+  with every null combination of the three gradients; the
   gate backward (both small kernels, the strided pair, colsum) against float64 on both sides of 768 tokens per block.
 * No-aux router: E = 32 to 512, K up to 32, lanes per group 1 to 8, no mask, tied group scores, negative-bias kept
   experts against masked zeros, the zero-score kept expert's gradient, NaN rows, refusals.
@@ -212,19 +213,46 @@ def permute_prepared(x, ids32, ws, E):
     return perm.check("permuted"), rmap.check("row_id_map")
 
 
-@pytest.mark.parametrize("E,T,H,Ks", [pytest.param(E, 1000, 256, range(1, E + 1), id=str(E)) for E in range(1, 9)] + [
-    pytest.param(8, 8192, 2048, (2,), id="bench")])
-def test_fused_gate_route_equals_router_on_its_own_logits(E, T, H, Ks):
+def _edge_gate_inputs(T, H, E):
+    """Two gate inputs (x, w) and (x, w') whose logits hold the router's edge rows.  The tensor-core gate splits the fp32
+    weight into three bf16 planes: powers of two leave the lower two planes zero, and w' = w but inf at experts 1 and 3
+    of column 0, which leaves inf - inf = NaN in them, so those two logits are NaN in every row of w'.  Row 0 of x is
+    zero (tied zeros), row 1 holds a NaN (a NaN row), rows 2 and 3 overflow to -inf and +inf at experts E-2 and E-1 and
+    the other way round, and row 4 has logits 3 and 2 at experts 0 and 2: [3, nan, 2, nan] under w' at E = 4."""
     x, w, _ = R.gate_inputs(T, H, E, "random", E, "cuda")
-    for K in Ks:
-        for scoring, norm, scaling in [("softmax", True, 1.0), ("sigmoid", False, 2.5), ("softmax", False, 2.5)]:
-            f = fused(x, w, K, scoring, norm, scaling)
-            r = router(f["logits"].clone(), K, scoring, norm, scaling, ws=True)
-            for k in ("rw", "tw", "ids", "i32", "tpe", "ws"):
-                assert torch.equal(f[k].view(torch.uint8) if f[k].dtype == torch.float32 else f[k],
-                                   r[k].view(torch.uint8) if r[k].dtype == torch.float32 else r[k]), (K, scoring, k)
-            (pf, mf), (pr, mr) = permute_prepared(x, f["i32"], f["ws"], E), permute_prepared(x, r["i32"], r["ws"], E)
-            assert torch.equal(mf, mr) and torch.equal(pf, pr), (K, scoring, "permuted rows")
+    x[:5] = 0
+    x[:, 1] = 0
+    x[1, 5] = float("nan")
+    x[2, 1], x[3, 1] = 2.0 ** 100, -(2.0 ** 100)
+    x[4, 2] = 1
+    w[:, 1] = 0
+    w[E - 2, 1], w[E - 1, 1] = -(2.0 ** 100), 2.0 ** 100
+    w[0, 2], w[2, 2] = 3, 2
+    w_nan = w.clone()
+    w_nan[[1, 3], 0] = float("inf")
+    return [(x, w), (x, w_nan)]
+
+
+@pytest.mark.parametrize("E,T,H,Ks,edges", [
+    pytest.param(E, 1000, 256, range(1, E + 1), False, id=str(E)) for E in range(1, 9)] + [
+    pytest.param(8, 8192, 2048, (2,), False, id="bench")] + [
+    pytest.param(E, 1000, 256, range(1, E + 1), True, id=f"edges{E}") for E in (4, 8)])
+def test_fused_gate_route_equals_router_on_its_own_logits(E, T, H, Ks, edges):
+    inputs = _edge_gate_inputs(T, H, E) if edges else [R.gate_inputs(T, H, E, "random", E, "cuda")[:2]]
+    for i, (x, w) in enumerate(inputs):
+        for K in Ks:
+            for scoring, norm, scaling in [("softmax", True, 1.0), ("sigmoid", False, 2.5), ("softmax", False, 2.5)]:
+                what = (i, K, scoring)
+                f = fused(x, w, K, scoring, norm, scaling)
+                r = router(f["logits"].clone(), K, scoring, norm, scaling, ws=True)
+                for k in ("rw", "tw", "ids", "i32", "tpe", "ws"):
+                    assert torch.equal(f[k].view(torch.uint8) if f[k].dtype == torch.float32 else f[k],
+                                       r[k].view(torch.uint8) if r[k].dtype == torch.float32 else r[k]), (*what, k)
+                (pf, mf), (pr, mr) = permute_prepared(x, f["i32"], f["ws"], E), permute_prepared(x, r["i32"], r["ws"], E)
+                assert torch.equal(mf, mr) and torch.equal(pf, pr), (*what, "permuted rows")
+                if edges and i == 1 and E == 4 and K == 3 and scoring == "sigmoid":
+                    # NaN at experts 1 and 3: the third pick falls back to the lowest id not selected yet
+                    assert f["ids"][4].tolist() == [0, 2, 1], f["ids"][4].tolist()
 
 
 # ---- greedy router ---------------------------------------------------------------------------------------------------
@@ -346,17 +374,20 @@ def test_router_gate_bwd_equals_the_two_calls(E, T, H, Ks):
     for K in Ks:
         scoring, norm, scaling = [("softmax", True, 1.0), ("sigmoid", False, 2.5)][K % 2]
         r = router(lg, K, scoring, norm, scaling)
-        g_tw, g_rw, g_dir = torch.randn(T, K, device="cuda"), torch.randn(T, E, device="cuda"), torch.randn(T, E, device="cuda")
         sc = 1 if scoring == "sigmoid" else 0
         ws = torch.empty(int(lib.xtb_gate_logits_bwd_workspace_bytes(T, H, E)), dtype=torch.uint8, device="cuda")
-        gw1, gx1 = torch.empty(E, H, device="cuda"), torch.empty(T, H, dtype=torch.bfloat16, device="cuda")
-        _ok(lib.xtb_router_gate_bwd(_p(r["rw"]), _p(r["tw"]), _p(r["ids"]), _p(g_tw), _p(g_rw), _p(g_dir), _p(x), _p(w),
-                                    _p(gw1), _p(gx1), T, H, E, K, sc, int(norm), scaling, _p(ws), _st()))
-        gl = greedy_bwd(r, K, scoring, norm, scaling, g_tw, g_rw, g_dir)
-        gw2, gx2 = torch.empty(E, H, device="cuda"), torch.empty(T, H, dtype=torch.bfloat16, device="cuda")
-        _ok(lib.xtb_gate_logits_bwd(_p(gl), _p(x), _p(w), _p(gw2), _p(gx2), None, T, H, E, _p(ws), _st()))
-        assert torch.equal(gw1.view(torch.int32), gw2.view(torch.int32)), K
-        assert torch.equal(gx1.view(torch.int16), gx2.view(torch.int16)), K
+        for mask in range(8):
+            g_tw = torch.randn(T, K, device="cuda") if mask & 1 else None
+            g_rw = torch.randn(T, E, device="cuda") if mask & 2 else None
+            g_dir = torch.randn(T, E, device="cuda") if mask & 4 else None
+            gw1, gx1 = torch.empty(E, H, device="cuda"), torch.empty(T, H, dtype=torch.bfloat16, device="cuda")
+            _ok(lib.xtb_router_gate_bwd(_p(r["rw"]), _p(r["tw"]), _p(r["ids"]), _p(g_tw), _p(g_rw), _p(g_dir), _p(x),
+                                        _p(w), _p(gw1), _p(gx1), T, H, E, K, sc, int(norm), scaling, _p(ws), _st()))
+            gl = greedy_bwd(r, K, scoring, norm, scaling, g_tw, g_rw, g_dir)
+            gw2, gx2 = torch.empty(E, H, device="cuda"), torch.empty(T, H, dtype=torch.bfloat16, device="cuda")
+            _ok(lib.xtb_gate_logits_bwd(_p(gl), _p(x), _p(w), _p(gw2), _p(gx2), None, T, H, E, _p(ws), _st()))
+            assert torch.equal(gw1.view(torch.int32), gw2.view(torch.int32)), (K, mask)
+            assert torch.equal(gx1.view(torch.int16), gx2.view(torch.int16)), (K, mask)
 
 
 @pytest.mark.parametrize("T", [1, 700, 20000, 250_000])

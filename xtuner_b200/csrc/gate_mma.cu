@@ -19,6 +19,7 @@
 // LDG.128, and a B fragment is simply 8 consecutive bf16 of one expert's row.
 #include "common.cuh"
 #include "dispatch_scan.cuh"
+#include "greedy_router.cuh"
 
 namespace xtb {
 
@@ -98,59 +99,9 @@ constexpr int kGateBatch = 8;     // 32-column steps whose loads are in flight t
 // ---- gate + greedy router + dispatch bucketing in ONE launch (xtb_gate_route_dispatch) -------------------------------
 // The tensor-core gate produces the logits of one 32-token block = one histogram chunk of the dispatch
 // (dispatch_scan.cuh: kChunkTokens == 32) in shared memory; routing those 32 tokens there (one thread per token, E <= 8:
-// the same arithmetic, in the same order, as router_greedy_kernel<1, 8> in route.cu) and counting the chunk's expert
-// histogram with ballots removes the separate router launch (12.7 us per layer at C2, all latency) and the logits
-// round trip.  The last block scans the chunk histograms exactly like the router kernel does.
-__device__ __forceinline__ void route_token_e8(const float* __restrict__ lg, int E, int K, int scoring, int norm_topk,
-                                               float scaling, float (&p)[8], float (&wv)[8], int (&se)[8]) {
-  float m = -INFINITY;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    p[j] = (j < E) ? lg[j] : -INFINITY;
-    m = fmaxf(m, p[j]);
-  }
-  if (scoring == XTB_SCORE_SOFTMAX) {
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      p[j] = (j < E) ? expf(p[j] - m) : 0.f;
-      s += p[j];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) p[j] = p[j] / s;
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) p[j] = (j < E) ? 1.f / (1.f + expf(-p[j])) : -INFINITY;
-  }
-  unsigned taken = 0;
-  float sum = 0.f;
-  for (int k = 0; k < K; ++k) {
-    float bv = -INFINITY;
-    int be = 0x7fffffff;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      if (!((taken >> j) & 1u) && j < E && (p[j] > bv)) {
-        bv = p[j];
-        be = j;
-      }
-    }
-    if (be < 0 || be >= E) {  // NaN rows: the lowest index not selected yet, as the router kernel does (at most k < E)
-      be = __ffs(~taken) - 1;
-      bv = 0.f;
-    }
-    taken |= 1u << be;
-    wv[k] = bv;
-    se[k] = be;
-    sum += bv;
-  }
-  for (int k = 0; k < K; ++k) {
-    float v = wv[k];
-    if (norm_topk) v = v / sum;
-    if (scaling != 1.0f) v = v * scaling;
-    wv[k] = v;
-  }
-}
-
+// greedy_route_token<1, 8>) and counting the chunk's expert histogram with ballots removes the separate router launch
+// (12.7 us per layer at C2, all latency) and the logits round trip.  The last block scans the chunk histograms exactly
+// like the router kernel does.
 __global__ void __launch_bounds__(256) gate_route_mma_kernel(
     const __nv_bfloat16* __restrict__ x, const float* __restrict__ w, float* __restrict__ logits, int T, int H, int E,
     int K, int scoring, int norm_topk, float scaling, float* __restrict__ router_weights,
@@ -228,7 +179,7 @@ __global__ void __launch_bounds__(256) gate_route_mma_kernel(
       const bool active = token < T;
       float pr[8], wv[8];
       int se[8];
-      route_token_e8(s_logit[lane], E, K, scoring, norm_topk, scaling, pr, wv, se);
+      greedy_route_token<1, 8>(s_logit[lane], 0, E, K, scoring, norm_topk, scaling, pr, wv, se);
       if (active) {
 #pragma unroll
         for (int j = 0; j < 8; ++j)

@@ -3,6 +3,7 @@
 // HBM/latency bound ([T,E] tensors), not tensor-core work.
 #include "common.cuh"
 #include "dispatch_scan.cuh"
+#include "greedy_router.cuh"
 
 namespace xtb {
 
@@ -256,9 +257,8 @@ __global__ void __launch_bounds__(E_MAX <= 8 ? 512 : 256) gate_bwd_small_kernel(
 }
 
 // a2 backward + a1 backward in one launch (xtb_router_gate_bwd; E <= 8): the prologue computes this block's
-// grad_logits rows from the router's saved outputs — same arithmetic, in the same order, as
-// router_greedy_bwd_kernel<1, 8> — straight into the shared-memory tile the gate backward streams from, so the
-// [T,E] grad_logits tensor and the 9.7 us router-backward launch disappear.
+// grad_logits rows from the router's saved outputs straight into the shared-memory tile the gate backward streams
+// from, so the [T,E] grad_logits tensor and the 9.7 us router-backward launch disappear.
 __global__ void __launch_bounds__(512) router_gate_bwd_kernel(
     const float* __restrict__ router_weights, const float* __restrict__ topk_weights,
     const int64_t* __restrict__ topk_ids, const float* __restrict__ g_tw, const float* __restrict__ g_rw,
@@ -272,48 +272,9 @@ __global__ void __launch_bounds__(512) router_gate_bwd_kernel(
   for (int tt = threadIdx.x; tt < tokens_per_block; tt += blockDim.x) {
     const int tok = t_begin + tt;
     float gl[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (tok < t_end) {
-      float p[8], gp[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        p[j] = (j < E) ? router_weights[(size_t)tok * E + j] : 0.f;
-        gp[j] = (j < E && g_rw) ? g_rw[(size_t)tok * E + j] : 0.f;
-      }
-      if (g_tw) {
-        float sm = 0.f, dot = 0.f;
-        for (int k = 0; k < K; ++k) {
-          const int id = (int)topk_ids[(size_t)tok * K + k];
-          const float g = g_tw[(size_t)tok * K + k];
-          const float twk = topk_weights[(size_t)tok * K + k];
-          float v = 0.f;
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (j == id) v = p[j];
-          sm += v;
-          dot += g * (scaling != 1.0f ? twk / scaling : twk);
-        }
-        for (int k = 0; k < K; ++k) {
-          const int id = (int)topk_ids[(size_t)tok * K + k];
-          const float g = g_tw[(size_t)tok * K + k];
-          const float gv = norm_topk ? scaling * (g - dot) / sm : scaling * g;
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (j == id) gp[j] += gv;
-        }
-      }
-      if (scoring == XTB_SCORE_SOFTMAX) {
-        float d = 0.f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) d = fmaf(gp[j], p[j], d);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) gl[j] = p[j] * (gp[j] - d);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) gl[j] = gp[j] * p[j] * (1.f - p[j]);
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) gl[j] = (j < E) ? gl[j] + (g_direct ? g_direct[(size_t)tok * E + j] : 0.f) : 0.f;
-    }
+    if (tok < t_end)
+      greedy_route_token_bwd<1, 8>(router_weights, topk_weights, topk_ids, g_tw, g_rw, g_direct, tok, 0, E, K, scoring,
+                                   norm_topk, scaling, gl);
 #pragma unroll
     for (int j = 0; j < 8; ++j) s_gl[tt * 8 + j] = gl[j];
   }
@@ -339,24 +300,9 @@ __global__ void colsum_kernel(const float* __restrict__ gl, float* __restrict__ 
 
 // =====================================================================================================
 // a2  greedy router.  LPT lanes cooperate on one token; each lane holds VPL consecutive experts
-// (e = sub*VPL + j).  Softmax follows torch's CUDA formulation (max, exp(x-max), sum, divide) in fp32.
-// Top-k = K rounds of (value desc, index asc) arg-max over the group: the order torch.topk(sorted=True)
-// returns on tie-free rows.  Histogram: warp-aggregated shared-memory counters, one global atomic per
-// (block, expert).
+// (e = sub*VPL + j); the per-token arithmetic is greedy_route_token (greedy_router.cuh).  Histogram:
+// warp-aggregated shared-memory counters, one global atomic per (block, expert).
 // =====================================================================================================
-template <int LPT, int VPL>
-__device__ __forceinline__ void group_argmax(float& best_v, int& best_e) {
-#pragma unroll
-  for (int o = LPT / 2; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, best_v, o);
-    const int oe = __shfl_xor_sync(0xffffffffu, best_e, o);
-    if (ov > best_v || (ov == best_v && oe < best_e)) {
-      best_v = ov;
-      best_e = oe;
-    }
-  }
-}
-
 template <int LPT, int VPL>
 __global__ void __launch_bounds__((LPT * 32 > 256) ? LPT * 32 : 256)
 router_greedy_kernel(const float* __restrict__ logits, int T, int E, int K, int scoring, int norm_topk, float scaling,
@@ -379,76 +325,19 @@ router_greedy_kernel(const float* __restrict__ logits, int T, int E, int K, int 
   const int sub = threadIdx.x % LPT;
   const bool active = token < T;
   const int tok = active ? token : T - 1;  // keep all lanes in the shuffles
-
-  float p[VPL];
   const int e0 = sub * VPL;
-  float m = -INFINITY;
-#pragma unroll
-  for (int j = 0; j < VPL; ++j) {
-    const int e = e0 + j;
-    p[j] = (e < E) ? logits[(size_t)tok * E + e] : -INFINITY;
-    m = fmaxf(m, p[j]);
-  }
-  if (scoring == XTB_SCORE_SOFTMAX) {
-#pragma unroll
-    for (int o = LPT / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < VPL; ++j) {
-      p[j] = (e0 + j < E) ? expf(p[j] - m) : 0.f;
-      s += p[j];
-    }
-#pragma unroll
-    for (int o = LPT / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-#pragma unroll
-    for (int j = 0; j < VPL; ++j) p[j] = p[j] / s;
-  } else {
-#pragma unroll
-    for (int j = 0; j < VPL; ++j) p[j] = (e0 + j < E) ? 1.f / (1.f + expf(-p[j])) : -INFINITY;
-  }
+
+  float p[VPL], sel_w[8];
+  int sel_e[8];
+  greedy_route_token<LPT, VPL>(logits + (size_t)tok * E, e0, E, K, scoring, norm_topk, scaling, p, sel_w, sel_e);
   if (active) {
 #pragma unroll
     for (int j = 0; j < VPL; ++j)
       if (e0 + j < E) router_weights[(size_t)token * E + e0 + j] = p[j];
   }
-
-  // top-k
-  unsigned taken = 0;  // bit j set: p[j] already selected
-  float sel_v[8];
-  int sel_e[8];
-  float sum = 0.f;
-  for (int k = 0; k < K; ++k) {
-    float bv = -INFINITY;
-    int be = 0x7fffffff;
-#pragma unroll
-    for (int j = 0; j < VPL; ++j) {
-      if (!((taken >> j) & 1u) && e0 + j < E && (p[j] > bv)) {
-        bv = p[j];
-        be = e0 + j;
-      }
-    }
-    group_argmax<LPT, VPL>(bv, be);
-    if (be < 0 || be >= E) {  // only reachable with NaN rows: the lowest index not selected yet.  sel_e is the same on
-                              // every lane of the group, and that index is at most k < K <= E.
-      unsigned used = 0;
-      for (int i = 0; i < k; ++i)
-        if (sel_e[i] < 32) used |= 1u << sel_e[i];
-      be = __ffs(~used) - 1;
-      bv = 0.f;
-    }
-    if (be >= e0 && be < e0 + VPL) taken |= 1u << (be - e0);
-    if (k < 8) {
-      sel_v[k] = bv;
-      sel_e[k] = be;
-    }
-    sum += bv;
-  }
   if (active && sub == 0) {
     for (int k = 0; k < K; ++k) {
-      float wv = sel_v[k];
-      if (norm_topk) wv = wv / sum;
-      if (scaling != 1.0f) wv = wv * scaling;
-      topk_weights[(size_t)token * K + k] = wv;
+      topk_weights[(size_t)token * K + k] = sel_w[k];
       topk_ids[(size_t)token * K + k] = (int64_t)sel_e[k];
       if (topk_ids_i32) topk_ids_i32[(size_t)token * K + k] = sel_e[k];
       if (chunk_counts) atomicAdd(&s_chunk[((threadIdx.x / LPT) / kChunkTokens) * E + sel_e[k]], 1);
@@ -485,55 +374,13 @@ __global__ void __launch_bounds__(256) router_greedy_bwd_kernel(
   const int tok = active ? token : T - 1;
   const int e0 = sub * VPL;
 
-  float p[VPL], gp[VPL];
-#pragma unroll
-  for (int j = 0; j < VPL; ++j) {
-    const int e = e0 + j;
-    p[j] = (e < E) ? router_weights[(size_t)tok * E + e] : 0.f;
-    gp[j] = (e < E && g_rw) ? g_rw[(size_t)tok * E + e] : 0.f;
-  }
-  if (g_tw) {
-    // s = sum of selected probabilities; dot = sum_k g_k * (v_k / s)
-    float s = 0.f, dot = 0.f;
-    for (int k = 0; k < K; ++k) {
-      const int id = (int)topk_ids[(size_t)tok * K + k];
-      const float g = g_tw[(size_t)tok * K + k];
-      const float twk = topk_weights[(size_t)tok * K + k];
-      float v = 0.f;
-      if (id >= e0 && id < e0 + VPL) v = p[id - e0];
-#pragma unroll
-      for (int o = LPT / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      s += v;
-      dot += g * (scaling != 1.0f ? twk / scaling : twk);  // twk/scaling == v_k/s when norm_topk
-    }
-    for (int k = 0; k < K; ++k) {
-      const int id = (int)topk_ids[(size_t)tok * K + k];
-      if (id >= e0 && id < e0 + VPL) {
-        const float g = g_tw[(size_t)tok * K + k];
-        const float gv = norm_topk ? scaling * (g - dot) / s : scaling * g;
-        gp[id - e0] += gv;
-      }
-    }
-  }
   float gl[VPL];
-  if (scoring == XTB_SCORE_SOFTMAX) {
-    float d = 0.f;
-#pragma unroll
-    for (int j = 0; j < VPL; ++j) d = fmaf(gp[j], p[j], d);
-#pragma unroll
-    for (int o = LPT / 2; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-#pragma unroll
-    for (int j = 0; j < VPL; ++j) gl[j] = p[j] * (gp[j] - d);
-  } else {
-#pragma unroll
-    for (int j = 0; j < VPL; ++j) gl[j] = gp[j] * p[j] * (1.f - p[j]);
-  }
+  greedy_route_token_bwd<LPT, VPL>(router_weights, topk_weights, topk_ids, g_tw, g_rw, g_direct, tok, e0, E, K, scoring,
+                                   norm_topk, scaling, gl);
   if (active) {
 #pragma unroll
-    for (int j = 0; j < VPL; ++j) {
-      const int e = e0 + j;
-      if (e < E) grad_logits[(size_t)token * E + e] = gl[j] + (g_direct ? g_direct[(size_t)token * E + e] : 0.f);
-    }
+    for (int j = 0; j < VPL; ++j)
+      if (e0 + j < E) grad_logits[(size_t)token * E + e0 + j] = gl[j];
   }
 }
 
