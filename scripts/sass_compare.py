@@ -17,6 +17,8 @@ def demangle(n): return subprocess.run(["c++filt",n],capture_output=True,text=Tr
 newd={demangle(k):k for k in new}
 def dropped(d):  # a template parameter removed together with its other value: <M, N, E, 1> -> <M, N, E>, f<true> -> f
     d=re.sub(r"<(\d+), (\d+), (\d+), 1>$", r"<\1, \2, \3>", d)
+    d=re.sub(r"(::rmsnorm_gate_kernel<\d+, \d+, \d+), true>$", r"\1>", d)  # the gate became unconditional
+    d=re.sub(r"(::dispatch_bwd_rmsnorm_kernel)<0, (\d+)>$", r"\1<\2>", d)  # runtime K only: KT = 0 went
     return re.sub(r"^void (\S+)<true>$", r"\1", d)
 same=diff=0
 for k,v in old.items():

@@ -108,6 +108,23 @@ __device__ __forceinline__ void unpack_bf16x2(uint32_t v, float& lo, float& hi) 
   hi = __uint_as_float(v & 0xffff0000u);
 }
 
+// one 16-byte vector of 8 bf16 <-> 8 floats, element j in f[j].  The vector is taken by reference, which leaves the
+// callers' generated code as it is with four unpack_bf16x2 calls.
+__device__ __forceinline__ void unpack_bf16x8(const uint4& v, float (&f)[8]) {
+  unpack_bf16x2(v.x, f[0], f[1]);
+  unpack_bf16x2(v.y, f[2], f[3]);
+  unpack_bf16x2(v.z, f[4], f[5]);
+  unpack_bf16x2(v.w, f[6], f[7]);
+}
+__device__ __forceinline__ uint4 pack_bf16x8(const float (&f)[8]) {
+  uint4 v;
+  v.x = pack_bf16x2(f[0], f[1]);
+  v.y = pack_bf16x2(f[2], f[3]);
+  v.z = pack_bf16x2(f[4], f[5]);
+  v.w = pack_bf16x2(f[6], f[7]);
+  return v;
+}
+
 // 16-byte streaming global accesses (read-once / write-once data: bypass L1 allocation)
 __device__ __forceinline__ uint4 ld_stream_16(const void* p) {
   uint4 r;

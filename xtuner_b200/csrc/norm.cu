@@ -15,22 +15,20 @@
 namespace xtb {
 
 
-// ---- forward: norm (+ optional gate logits).  A warp owns TW tokens whose rows stay in registers (ROW8 16-byte
-// vectors per lane and token): one HBM read, all loads of the rows in flight at once, W_gate resident in smem ------
-template <int E_MAX, int TW, int ROW8, bool WITH_GATE>
-__global__ void __launch_bounds__(256, WITH_GATE ? 1 : 3) rmsnorm_gate_kernel(const __nv_bfloat16* __restrict__ h,
+// ---- forward: norm + gate logits.  A warp owns TW tokens whose rows stay in registers (ROW8 16-byte vectors per lane
+// and token): one HBM read, all loads of the rows in flight at once, W_gate resident in smem ------------------------
+template <int E_MAX, int TW, int ROW8>
+__global__ void __launch_bounds__(256, 1) rmsnorm_gate_kernel(const __nv_bfloat16* __restrict__ h,
                                                               const float* __restrict__ norm_w,  // [H] fp32
                                                               const float* __restrict__ gate_w,  // [E,H] fp32
                                                               __nv_bfloat16* __restrict__ x_out,
                                                               float* __restrict__ rstd_out, float* __restrict__ logits,
                                                               int T, int H, int E, float eps) {
-  extern __shared__ float s_w[];  // gate weight [E][H] (WITH_GATE) followed by norm weight [H]
-  float* s_nw = s_w + (WITH_GATE ? (size_t)E * H : 0);
-  if (WITH_GATE) {
-    const float4* src = reinterpret_cast<const float4*>(gate_w);
-    float4* dst = reinterpret_cast<float4*>(s_w);
-    for (int i = threadIdx.x; i < E * H / 4; i += blockDim.x) dst[i] = __ldg(src + i);
-  }
+  extern __shared__ float s_w[];  // gate weight [E][H] followed by norm weight [H]
+  float* s_nw = s_w + (size_t)E * H;
+  const float4* src = reinterpret_cast<const float4*>(gate_w);
+  float4* dst = reinterpret_cast<float4*>(s_w);
+  for (int i = threadIdx.x; i < E * H / 4; i += blockDim.x) dst[i] = __ldg(src + i);
   for (int i = threadIdx.x; i < H; i += blockDim.x) s_nw[i] = norm_w[i];
   __syncthreads();
   const int lane = threadIdx.x & 31;
@@ -51,10 +49,7 @@ __global__ void __launch_bounds__(256, WITH_GATE ? 1 : 3) rmsnorm_gate_kernel(co
       float ss = 0.f;
 #pragma unroll
       for (int c = 0; c < ROW8; ++c) {
-        unpack_bf16x2(raw[i][c].x, xv[i][c][0], xv[i][c][1]);
-        unpack_bf16x2(raw[i][c].y, xv[i][c][2], xv[i][c][3]);
-        unpack_bf16x2(raw[i][c].z, xv[i][c][4], xv[i][c][5]);
-        unpack_bf16x2(raw[i][c].w, xv[i][c][6], xv[i][c][7]);
+        unpack_bf16x8(raw[i][c], xv[i][c]);
 #pragma unroll
         for (int j = 0; j < 8; ++j) ss = fmaf(xv[i][c][j], xv[i][c][j], ss);
       }
@@ -82,38 +77,34 @@ __global__ void __launch_bounds__(256, WITH_GATE ? 1 : 3) rmsnorm_gate_kernel(co
         }
         if (t0 + i < T) st_stream_16(x_out + (size_t)(t0 + i) * H + hh, make_uint4(p[0], p[1], p[2], p[3]));
       }
-      if (WITH_GATE) {
 #pragma unroll
-        for (int e = 0; e < E_MAX; ++e) {
-          if (e < E) {
-            const float4 w0 = *reinterpret_cast<const float4*>(s_w + (size_t)e * H + hh);
-            const float4 w1 = *reinterpret_cast<const float4*>(s_w + (size_t)e * H + hh + 4);
+      for (int e = 0; e < E_MAX; ++e) {
+        if (e < E) {
+          const float4 w0 = *reinterpret_cast<const float4*>(s_w + (size_t)e * H + hh);
+          const float4 w1 = *reinterpret_cast<const float4*>(s_w + (size_t)e * H + hh + 4);
 #pragma unroll
-            for (int i = 0; i < TW; ++i) {
-              float a = acc[i][e];
-              a = fmaf(xv[i][c][0], w0.x, a);
-              a = fmaf(xv[i][c][1], w0.y, a);
-              a = fmaf(xv[i][c][2], w0.z, a);
-              a = fmaf(xv[i][c][3], w0.w, a);
-              a = fmaf(xv[i][c][4], w1.x, a);
-              a = fmaf(xv[i][c][5], w1.y, a);
-              a = fmaf(xv[i][c][6], w1.z, a);
-              a = fmaf(xv[i][c][7], w1.w, a);
-              acc[i][e] = a;
-            }
+          for (int i = 0; i < TW; ++i) {
+            float a = acc[i][e];
+            a = fmaf(xv[i][c][0], w0.x, a);
+            a = fmaf(xv[i][c][1], w0.y, a);
+            a = fmaf(xv[i][c][2], w0.z, a);
+            a = fmaf(xv[i][c][3], w0.w, a);
+            a = fmaf(xv[i][c][4], w1.x, a);
+            a = fmaf(xv[i][c][5], w1.y, a);
+            a = fmaf(xv[i][c][6], w1.z, a);
+            a = fmaf(xv[i][c][7], w1.w, a);
+            acc[i][e] = a;
           }
         }
       }
     }
-    if (WITH_GATE) {
 #pragma unroll
-      for (int i = 0; i < TW; ++i)
+    for (int i = 0; i < TW; ++i)
 #pragma unroll
-        for (int e = 0; e < E_MAX; ++e) {
-          const float s = warp_sum(acc[i][e]);
-          if (lane == 0 && e < E && t0 + i < T) logits[(size_t)(t0 + i) * E + e] = s;
-        }
-    }
+      for (int e = 0; e < E_MAX; ++e) {
+        const float s = warp_sum(acc[i][e]);
+        if (lane == 0 && e < E && t0 + i < T) logits[(size_t)(t0 + i) * E + e] = s;
+      }
   }
 }
 
@@ -159,10 +150,7 @@ __global__ void __launch_bounds__(256) rmsnorm_cols_kernel(const __nv_bfloat16* 
     for (int i = 0; i < TB; ++i) {
       raw[i] = (c < H && t0 + i < T) ? ld_stream_16(h + (size_t)(t0 + i) * H + c) : make_uint4(0, 0, 0, 0);
       float f[8];
-      unpack_bf16x2(raw[i].x, f[0], f[1]);
-      unpack_bf16x2(raw[i].y, f[2], f[3]);
-      unpack_bf16x2(raw[i].z, f[4], f[5]);
-      unpack_bf16x2(raw[i].w, f[6], f[7]);
+      unpack_bf16x8(raw[i], f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) ss[i] = fmaf(f[j], f[j], ss[i]);
     }
@@ -185,10 +173,7 @@ __global__ void __launch_bounds__(256) rmsnorm_cols_kernel(const __nv_bfloat16* 
       if (t0 + i >= T) continue;
       const uint4 r = (n_pass == 1) ? raw[i] : ld_stream_16(h + (size_t)(t0 + i) * H + c);
       float f[8];
-      unpack_bf16x2(r.x, f[0], f[1]);
-      unpack_bf16x2(r.y, f[2], f[3]);
-      unpack_bf16x2(r.z, f[4], f[5]);
-      unpack_bf16x2(r.w, f[6], f[7]);
+      unpack_bf16x8(r, f);
       uint4 o;
       o.x = pack_bf16x2(f[0] * rstd[i] * nw[0], f[1] * rstd[i] * nw[1]);
       o.y = pack_bf16x2(f[2] * rstd[i] * nw[2], f[3] * rstd[i] * nw[3]);
@@ -207,40 +192,90 @@ __global__ void __launch_bounds__(256) rmsnorm_cols_kernel(const __nv_bfloat16* 
 // Column-owned and persistent: thread j owns columns [8j, 8j+8) (H == 2048 per pass of 256 threads), a block walks
 // over groups of TB tokens; the per-token row reduction is a block reduction, the per-column weight gradient lives
 // in 8 registers per thread for the whole kernel (no atomics).  H must be <= 2048 and a multiple of 8.
-template <int KT, int TB>
-__global__ void __launch_bounds__(256, 2) dispatch_bwd_rmsnorm_kernel(
-    const uint4* __restrict__ g_xp, const int32_t* __restrict__ row_id_map, const uint4* __restrict__ g_x_gate,
-    const uint4* __restrict__ h, const float* __restrict__ rstd, const float* __restrict__ norm_w,
-    const uint4* __restrict__ g_res, uint4* __restrict__ g_h, float* __restrict__ partial_gw, int T, int K_rt, int H) {
-  pdl_sync();
-  __shared__ float s_red[8 * TB];
-  const int K = KT > 0 ? KT : K_rt;
-  const int row_vec = H / 8;
-  const int v = threadIdx.x;           // 16-byte vector index inside the row
-  const bool live = v < row_vec;
-  float nw[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+// The two kernels below differ only in how a token's rows reach registers; the arithmetic is these four functions.
+// They keep no local arrays: their results go to arrays the caller owns, which also serve as their scratch.  A local
+// array in an inlined helper changes how nvcc allocates the kernels' registers.
+
+// the thread's 8 norm-weight columns (zeros past the end of the row)
+__device__ __forceinline__ void load_norm_w8(const float* norm_w, int v, bool live, float (&nw)[8]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) nw[j] = 0.f;
   if (live) {
     const float4 w0 = __ldg(reinterpret_cast<const float4*>(norm_w + v * 8));
     const float4 w1 = __ldg(reinterpret_cast<const float4*>(norm_w + v * 8 + 4));
     nw[0] = w0.x; nw[1] = w0.y; nw[2] = w0.z; nw[3] = w0.w; nw[4] = w1.x; nw[5] = w1.y; nw[6] = w1.z; nw[7] = w1.w;
   }
+}
+
+// One token before the row reduction: acc = fp32 sum of its K gathered rows, hv / gv / rs = its h, gate grad and rstd.
+// Adds the token's share of the norm-weight gradient to gw, returns wg in g (which holds the unpacked gate grad until
+// then), float(h) in hf and this thread's part of the row dot sum(wg * h).  A token past T (tok_ok false) contributes
+// zeros.
+__device__ __forceinline__ float norm_bwd_token(const float (&acc)[8], const uint4& hv, const uint4& gv, float rs,
+                                                bool has_gate, bool tok_ok, const float (&nw)[8], float (&gw)[8],
+                                                float (&g)[8], float (&hf)[8]) {
+  unpack_bf16x8(gv, g);
+  unpack_bf16x8(hv, hf);
+  float dot = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    float gj = __bfloat162float(__float2bfloat16_rn(acc[j]));               // permute-bwd output (bf16)
+    if (has_gate) gj = __bfloat162float(__float2bfloat16_rn(gj + g[j]));  // autograd's bf16 add
+    if (!tok_ok) gj = 0.f;
+    gw[j] = fmaf(gj * rs, hf[j], gw[j]);
+    gj *= nw[j];
+    g[j] = gj;
+    dot = fmaf(gj, hf[j], dot);
+  }
+  return dot;
+}
+
+// One token after the row reduction (dot = the whole row's sum): the token's 8 g_h values in o, before the bf16 pack,
+// with the residual grad rv added when has_res (o holds the unpacked rv until then)
+__device__ __forceinline__ void norm_bwd_token_out(const float (&g)[8], const float (&hf)[8], float dot, float rs,
+                                                   const uint4& rv, bool has_res, int H, float (&o)[8]) {
+  const float cterm = dot * rs * rs / (float)H;
+  unpack_bf16x8(rv, o);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    float val = (g[j] - hf[j] * cterm) * rs;
+    if (has_res) val = __bfloat162float(__float2bfloat16_rn(val)) + o[j];
+    o[j] = val;
+  }
+}
+
+// the block's row of norm-weight-gradient partials (reduced by reduce_partial_rows_kernel)
+__device__ __forceinline__ void store_partial_gw(float* __restrict__ partial_gw, int H, int v, bool live,
+                                                 const float (&gw)[8]) {
+  if (partial_gw && live) {
+    float* dst = partial_gw + (size_t)blockIdx.x * H + v * 8;
+    *reinterpret_cast<float4*>(dst) = make_float4(gw[0], gw[1], gw[2], gw[3]);
+    *reinterpret_cast<float4*>(dst + 4) = make_float4(gw[4], gw[5], gw[6], gw[7]);
+  }
+}
+
+// any K: a group's h / gate-grad / residual-grad vectors are loaded up front, the K rows of a token one after another
+template <int TB>
+__global__ void __launch_bounds__(256, 2) dispatch_bwd_rmsnorm_kernel(
+    const uint4* __restrict__ g_xp, const int32_t* __restrict__ row_id_map, const uint4* __restrict__ g_x_gate,
+    const uint4* __restrict__ h, const float* __restrict__ rstd, const float* __restrict__ norm_w,
+    const uint4* __restrict__ g_res, uint4* __restrict__ g_h, float* __restrict__ partial_gw, int T, int K, int H) {
+  pdl_sync();
+  __shared__ float s_red[8 * TB];
+  const int row_vec = H / 8;
+  const int v = threadIdx.x;           // 16-byte vector index inside the row
+  const bool live = v < row_vec;
+  float nw[8];
+  load_norm_w8(norm_w, v, live, nw);
   float gw[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   const int n_groups = (T + TB - 1) / TB;
   for (int grp = blockIdx.x; grp < n_groups; grp += gridDim.x) {
     const int t0 = grp * TB;
-    constexpr int KU = KT > 0 ? KT : 1;
-    uint4 rows[TB][KU], hv[TB], gv[TB], rv[TB];
+    uint4 hv[TB], gv[TB], rv[TB];
     float rs[TB];
 #pragma unroll
     for (int i = 0; i < TB; ++i) {
       const int t = min(t0 + i, T - 1);
-      if constexpr (KT > 0) {
-#pragma unroll
-        for (int k = 0; k < KT; ++k) {
-          const int r = row_id_map[(size_t)t * KT + k];
-          rows[i][k] = (live && r >= 0) ? ld_stream_16(g_xp + (size_t)r * row_vec + v) : make_uint4(0, 0, 0, 0);
-        }
-      }
       hv[i] = live ? ld_stream_16(h + (size_t)t * row_vec + v) : make_uint4(0, 0, 0, 0);
       gv[i] = (live && g_x_gate) ? ld_stream_16(g_x_gate + (size_t)t * row_vec + v) : make_uint4(0, 0, 0, 0);
       rv[i] = (live && g_res) ? ld_stream_16(g_res + (size_t)t * row_vec + v) : make_uint4(0, 0, 0, 0);
@@ -250,84 +285,27 @@ __global__ void __launch_bounds__(256, 2) dispatch_bwd_rmsnorm_kernel(
 #pragma unroll
     for (int i = 0; i < TB; ++i) {
       float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      if constexpr (KT > 0) {
+      const int t = min(t0 + i, T - 1);
+      for (int k = 0; k < K; ++k) {
+        const int r = row_id_map[(size_t)t * K + k];
+        if (!live || r < 0) continue;
+        float f[8];
+        unpack_bf16x8(ld_stream_16(g_xp + (size_t)r * row_vec + v), f);
 #pragma unroll
-        for (int k = 0; k < KT; ++k) {
-          float f[8];
-          unpack_bf16x2(rows[i][k].x, f[0], f[1]);
-          unpack_bf16x2(rows[i][k].y, f[2], f[3]);
-          unpack_bf16x2(rows[i][k].z, f[4], f[5]);
-          unpack_bf16x2(rows[i][k].w, f[6], f[7]);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) acc[j] += f[j];
-        }
-      } else {
-        const int t = min(t0 + i, T - 1);
-        for (int k = 0; k < K; ++k) {
-          const int r = row_id_map[(size_t)t * K + k];
-          if (!live || r < 0) continue;
-          const uint4 rr = ld_stream_16(g_xp + (size_t)r * row_vec + v);
-          float f[8];
-          unpack_bf16x2(rr.x, f[0], f[1]);
-          unpack_bf16x2(rr.y, f[2], f[3]);
-          unpack_bf16x2(rr.z, f[4], f[5]);
-          unpack_bf16x2(rr.w, f[6], f[7]);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) acc[j] += f[j];
-        }
+        for (int j = 0; j < 8; ++j) acc[j] += f[j];
       }
-      float gg[8];
-      unpack_bf16x2(gv[i].x, gg[0], gg[1]);
-      unpack_bf16x2(gv[i].y, gg[2], gg[3]);
-      unpack_bf16x2(gv[i].z, gg[4], gg[5]);
-      unpack_bf16x2(gv[i].w, gg[6], gg[7]);
-      unpack_bf16x2(hv[i].x, hf[i][0], hf[i][1]);
-      unpack_bf16x2(hv[i].y, hf[i][2], hf[i][3]);
-      unpack_bf16x2(hv[i].z, hf[i][4], hf[i][5]);
-      unpack_bf16x2(hv[i].w, hf[i][6], hf[i][7]);
-      dot[i] = 0.f;
-      const bool tok_ok = t0 + i < T;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float gj = __bfloat162float(__float2bfloat16_rn(acc[j]));                    // permute-bwd output (bf16)
-        if (g_x_gate) gj = __bfloat162float(__float2bfloat16_rn(gj + gg[j]));       // autograd's bf16 add
-        if (!tok_ok) gj = 0.f;
-        gw[j] = fmaf(gj * rs[i], hf[i][j], gw[j]);
-        gj *= nw[j];
-        g[i][j] = gj;
-        dot[i] = fmaf(gj, hf[i][j], dot[i]);
-      }
+      dot[i] = norm_bwd_token(acc, hv[i], gv[i], rs[i], g_x_gate != nullptr, t0 + i < T, nw, gw, g[i], hf[i]);
     }
     block_sum<TB>(dot, s_red);
 #pragma unroll
     for (int i = 0; i < TB; ++i) {
       if (!live || t0 + i >= T) continue;
-      const float cterm = dot[i] * rs[i] * rs[i] / (float)H;
-      float rr[8];
-      unpack_bf16x2(rv[i].x, rr[0], rr[1]);
-      unpack_bf16x2(rv[i].y, rr[2], rr[3]);
-      unpack_bf16x2(rv[i].z, rr[4], rr[5]);
-      unpack_bf16x2(rv[i].w, rr[6], rr[7]);
       float o[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float val = (g[i][j] - hf[i][j] * cterm) * rs[i];
-        if (g_res) val = __bfloat162float(__float2bfloat16_rn(val)) + rr[j];
-        o[j] = val;
-      }
-      uint4 ov;
-      ov.x = pack_bf16x2(o[0], o[1]);
-      ov.y = pack_bf16x2(o[2], o[3]);
-      ov.z = pack_bf16x2(o[4], o[5]);
-      ov.w = pack_bf16x2(o[6], o[7]);
-      st_stream_16(g_h + (size_t)(t0 + i) * row_vec + v, ov);
+      norm_bwd_token_out(g[i], hf[i], dot[i], rs[i], rv[i], g_res != nullptr, H, o);
+      st_stream_16(g_h + (size_t)(t0 + i) * row_vec + v, pack_bf16x8(o));
     }
   }
-  if (partial_gw && live) {
-    float* dst = partial_gw + (size_t)blockIdx.x * H + v * 8;
-    *reinterpret_cast<float4*>(dst) = make_float4(gw[0], gw[1], gw[2], gw[3]);
-    *reinterpret_cast<float4*>(dst + 4) = make_float4(gw[4], gw[5], gw[6], gw[7]);
-  }
+  store_partial_gw(partial_gw, H, v, live, gw);
 }
 
 // ---- the same backward with the loads of the NEXT token group in flight while the current one is reduced --------------
@@ -336,9 +314,9 @@ __global__ void __launch_bounds__(256, 2) dispatch_bwd_rmsnorm_kernel(
 // of DRAM peak, 24 % warps active).  Here every thread copies its own 16-byte pieces of group g+1 into a second
 // shared-memory stage with cp.async (LDGSTS: no registers held, no barrier needed — a thread only ever reads back what it
 // copied itself) before it touches group g; the row ids and rstd of group g+2 are fetched into registers at the same time so
-// that the address of a gathered row is never a load away when its copy is issued.  Arithmetic and summation order are
-// those of the kernel above: identical bits.  KT = top-k (compile time), TB tokens per group; dynamic smem =
-// 2 stages x TB x (KT + 3) pieces x 4 KiB.
+// that the address of a gathered row is never a load away when its copy is issued.  The arithmetic is the kernel above's
+// (the same functions, the same summation order): identical bits.  KT = top-k (compile time), TB tokens per group;
+// dynamic smem = 2 stages x TB x (KT + 3) pieces x 4 KiB.
 __device__ __forceinline__ void cp_async_16_zfill(void* smem_dst, const void* gsrc, bool pred) {
   const uint32_t dst = (uint32_t)__cvta_generic_to_shared(smem_dst);
   const int n = pred ? 16 : 0;  // src-size 0: nothing is read, 16 zero bytes are written
@@ -362,12 +340,8 @@ __global__ void __launch_bounds__(256, 2) dispatch_bwd_rmsnorm_pipe_kernel(
   const int row_vec = H / 8;
   const int v = threadIdx.x;
   const bool live = v < row_vec;
-  float nw[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  if (live) {
-    const float4 w0 = __ldg(reinterpret_cast<const float4*>(norm_w + v * 8));
-    const float4 w1 = __ldg(reinterpret_cast<const float4*>(norm_w + v * 8 + 4));
-    nw[0] = w0.x; nw[1] = w0.y; nw[2] = w0.z; nw[3] = w0.w; nw[4] = w1.x; nw[5] = w1.y; nw[6] = w1.z; nw[7] = w1.w;
-  }
+  float nw[8];
+  load_norm_w8(norm_w, v, live, nw);
   float gw[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   const int n_groups = (T + TB - 1) / TB;
   auto slot = [&](int stage, int i, int p) -> uint4* { return s_stage + ((size_t)((stage * TB + i) * P + p)) * 256 + v; };
@@ -424,62 +398,21 @@ __global__ void __launch_bounds__(256, 2) dispatch_bwd_rmsnorm_pipe_kernel(
       float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll
       for (int k = 0; k < KT; ++k) {
-        const uint4 rr = *slot(stage, i, k);
         float f[8];
-        unpack_bf16x2(rr.x, f[0], f[1]);
-        unpack_bf16x2(rr.y, f[2], f[3]);
-        unpack_bf16x2(rr.z, f[4], f[5]);
-        unpack_bf16x2(rr.w, f[6], f[7]);
+        unpack_bf16x8(*slot(stage, i, k), f);
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[j] += f[j];
       }
       const uint4 hv = *slot(stage, i, KT), gv = *slot(stage, i, KT + 1);
-      float gg[8];
-      unpack_bf16x2(gv.x, gg[0], gg[1]);
-      unpack_bf16x2(gv.y, gg[2], gg[3]);
-      unpack_bf16x2(gv.z, gg[4], gg[5]);
-      unpack_bf16x2(gv.w, gg[6], gg[7]);
-      unpack_bf16x2(hv.x, hf[i][0], hf[i][1]);
-      unpack_bf16x2(hv.y, hf[i][2], hf[i][3]);
-      unpack_bf16x2(hv.z, hf[i][4], hf[i][5]);
-      unpack_bf16x2(hv.w, hf[i][6], hf[i][7]);
-      dot[i] = 0.f;
-      const bool tok_ok = t0 + i < T;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float gj = __bfloat162float(__float2bfloat16_rn(acc[j]));                    // permute-bwd output (bf16)
-        if (g_x_gate) gj = __bfloat162float(__float2bfloat16_rn(gj + gg[j]));       // autograd's bf16 add
-        if (!tok_ok) gj = 0.f;
-        gw[j] = fmaf(gj * rs_cur[i], hf[i][j], gw[j]);
-        gj *= nw[j];
-        g[i][j] = gj;
-        dot[i] = fmaf(gj, hf[i][j], dot[i]);
-      }
+      dot[i] = norm_bwd_token(acc, hv, gv, rs_cur[i], g_x_gate != nullptr, t0 + i < T, nw, gw, g[i], hf[i]);
     }
     block_sum<TB>(dot, s_red);
 #pragma unroll
     for (int i = 0; i < TB; ++i) {
       if (!live || t0 + i >= T) continue;
-      const float cterm = dot[i] * rs_cur[i] * rs_cur[i] / (float)H;
-      const uint4 rv = *slot(stage, i, KT + 2);
-      float rr[8];
-      unpack_bf16x2(rv.x, rr[0], rr[1]);
-      unpack_bf16x2(rv.y, rr[2], rr[3]);
-      unpack_bf16x2(rv.z, rr[4], rr[5]);
-      unpack_bf16x2(rv.w, rr[6], rr[7]);
       float o[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float val = (g[i][j] - hf[i][j] * cterm) * rs_cur[i];
-        if (g_res) val = __bfloat162float(__float2bfloat16_rn(val)) + rr[j];
-        o[j] = val;
-      }
-      uint4 ov;
-      ov.x = pack_bf16x2(o[0], o[1]);
-      ov.y = pack_bf16x2(o[2], o[3]);
-      ov.z = pack_bf16x2(o[4], o[5]);
-      ov.w = pack_bf16x2(o[6], o[7]);
-      st_stream_16(g_h + (size_t)(t0 + i) * row_vec + v, ov);
+      norm_bwd_token_out(g[i], hf[i], dot[i], rs_cur[i], *slot(stage, i, KT + 2), g_res != nullptr, H, o);
+      st_stream_16(g_h + (size_t)(t0 + i) * row_vec + v, pack_bf16x8(o));
     }
 #pragma unroll
     for (int i = 0; i < TB; ++i) {
@@ -491,11 +424,7 @@ __global__ void __launch_bounds__(256, 2) dispatch_bwd_rmsnorm_pipe_kernel(
     stage ^= 1;
     grp = g1;
   }
-  if (partial_gw && live) {
-    float* dst = partial_gw + (size_t)blockIdx.x * H + v * 8;
-    *reinterpret_cast<float4*>(dst) = make_float4(gw[0], gw[1], gw[2], gw[3]);
-    *reinterpret_cast<float4*>(dst + 4) = make_float4(gw[4], gw[5], gw[6], gw[7]);
-  }
+  store_partial_gw(partial_gw, H, v, live, gw);
 }
 
 static int norm_bwd_blocks(int T) { return max(1, min(sm_count() * 2, (T + 3) / 4)); }  // 2 resident CTAs per SM
@@ -524,23 +453,18 @@ extern "C" int xtb_rmsnorm_gate(const void* h_bf16, const float* norm_w_f32, con
     return XTB_OK;
   }
   const int blocks = min(sm_count(), (T + 15) / 16);
-  const size_t smem = ((gate_w_f32 ? (size_t)E * H : 0) + H) * sizeof(float);
+  const size_t smem = ((size_t)E * H + H) * sizeof(float);
   XTB_CHECK_ARG(smem <= 200 * 1024, "xtb_rmsnorm_gate: E*H too large for the fused gate (%zu bytes of smem)", smem);
 #define XTB_RG(R8)                                                                                                   \
   do {                                                                                                               \
-    if (gate_w_f32) {                                                                                                \
-      static bool attr = false;                                                                                      \
-      if (!attr) {                                                                                                   \
-        XTB_CUDA(cudaFuncSetAttribute(rmsnorm_gate_kernel<8, 2, R8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                      200 * 1024));                                                                  \
-        attr = true;                                                                                                 \
-      }                                                                                                              \
-      rmsnorm_gate_kernel<8, 2, R8, true><<<blocks, 256, smem, st>>>(hp, norm_w_f32, gate_w_f32, xp, rstd_out, logits, T, \
-                                                                     H, E, eps);                                     \
-    } else {                                                                                                         \
-      rmsnorm_gate_kernel<1, 2, R8, false><<<blocks, 256, smem, st>>>(hp, norm_w_f32, nullptr, xp, rstd_out, nullptr, T, \
-                                                                      H, 0, eps);                                    \
+    static bool attr = false;                                                                                        \
+    if (!attr) {                                                                                                     \
+      XTB_CUDA(cudaFuncSetAttribute(rmsnorm_gate_kernel<8, 2, R8>, cudaFuncAttributeMaxDynamicSharedMemorySize,      \
+                                    200 * 1024));                                                                    \
+      attr = true;                                                                                                   \
     }                                                                                                                \
+    rmsnorm_gate_kernel<8, 2, R8><<<blocks, 256, smem, st>>>(hp, norm_w_f32, gate_w_f32, xp, rstd_out, logits, T, H, E, \
+                                                             eps);                                                   \
   } while (0)
   switch (H / 256) {
     case 1: XTB_RG(1); break;
@@ -571,11 +495,6 @@ extern "C" int xtb_moe_dispatch_bwd_rmsnorm(const void* g_xperm_bf16, const int3
   cudaStream_t st = as_stream(stream);
   const int blocks = norm_bwd_blocks(T);
   float* partial = g_norm_w ? static_cast<float*>(workspace) : nullptr;
-#define XTB_NB(KT)                                                                                                  \
-  XTB_CUDA(launch_pdl(dispatch_bwd_rmsnorm_kernel<KT, 4>, dim3(blocks), dim3(256), 0, st,                                                         \
-      static_cast<const uint4*>(g_xperm_bf16), row_id_map, static_cast<const uint4*>(g_x_gate_bf16),                 \
-      static_cast<const uint4*>(h_bf16), rstd, norm_w_f32, static_cast<const uint4*>(g_res_bf16),                    \
-      static_cast<uint4*>(g_h_bf16), partial, T, K, H))
 #define XTB_NBP(KT, TB)                                                                                             \
   do {                                                                                                               \
     constexpr size_t smem = (size_t)2 * TB * (KT + 3) * 256 * sizeof(uint4);                                         \
@@ -591,9 +510,12 @@ extern "C" int xtb_moe_dispatch_bwd_rmsnorm(const void* g_xperm_bf16, const int3
   } while (0)
   if (K == 2) XTB_NBP(2, 2);
   else if (K == 8) XTB_NBP(8, 1);
-  else XTB_NB(0);
+  else
+    XTB_CUDA(launch_pdl(dispatch_bwd_rmsnorm_kernel<4>, dim3(blocks), dim3(256), 0, st,
+                        static_cast<const uint4*>(g_xperm_bf16), row_id_map, static_cast<const uint4*>(g_x_gate_bf16),
+                        static_cast<const uint4*>(h_bf16), rstd, norm_w_f32, static_cast<const uint4*>(g_res_bf16),
+                        static_cast<uint4*>(g_h_bf16), partial, T, K, H));
 #undef XTB_NBP
-#undef XTB_NB
   XTB_LAUNCH_OK();
   if (g_norm_w) {
     // H outputs, up to 2 partial rows per SM: 32 warps per block put all of a lane's ~9 loads in flight at once

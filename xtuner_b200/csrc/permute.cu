@@ -46,6 +46,31 @@ __global__ void __launch_bounds__(256) permute_count_scan_kernel(const int32_t* 
 }
 
 // ---- kernel B: per-chunk stable ranks -> maps, then the row gather/scatter ---------------------------
+// The index work of one block (sub-chunk `sub` of chunk `c`), shared by both scatter kernels: the chunk's ids up to the
+// end of the sub-chunk into s_ids, then each entry's stable rank among the preceding entries of its chunk gives its
+// destination row, written to s_dest (for the row movement), row_id_map and sorted_indices.  Ends on a barrier.
+__device__ __forceinline__ void scatter_index(const int32_t* __restrict__ ids, int T, int K, int E, int c, int sub,
+                                              const int* __restrict__ counts, const int* __restrict__ expert_start,
+                                              int* s_ids, int* s_dest, int32_t* __restrict__ row_id_map,
+                                              int64_t* __restrict__ sorted_indices) {
+  const int64_t fc = (int64_t)c * kChunkTokens * K;  // first flat index of the chunk
+  const int base = sub * kSubTokens * K;             // entries of the chunk that precede this block
+  const int n_mine = (int)min((int64_t)kSubTokens * K, (int64_t)T * K - (fc + base));
+  const int n_load = base + n_mine;
+  for (int j = threadIdx.x; j < n_load; j += blockDim.x) s_ids[j] = ids[fc + j];
+  __syncthreads();
+  for (int j = threadIdx.x; j < n_mine; j += blockDim.x) {
+    const int e = s_ids[base + j];
+    int rank = 0;
+    for (int i = 0; i < base + j; ++i) rank += (s_ids[i] == e);
+    const int dest = (e >= 0 && e < E) ? expert_start[e] + counts[(size_t)c * E + e] + rank : -1;
+    s_dest[j] = dest;
+    row_id_map[fc + base + j] = dest;
+    if (sorted_indices && dest >= 0) sorted_indices[dest] = fc + base + j;
+  }
+  __syncthreads();
+}
+
 // One block per sub-chunk.  The rows pass through registers: the path for rows too long to stage kSubTokens of in shared
 // memory (kernel B' below).
 __global__ void __launch_bounds__(128) permute_scatter_kernel(const uint4* __restrict__ x,
@@ -63,25 +88,8 @@ __global__ void __launch_bounds__(128) permute_scatter_kernel(const uint4* __res
   const int sub = blockIdx.x % kSubPerChunk;         // sub-chunk inside it
   const int t0 = c * kChunkTokens + sub * kSubTokens;  // first token of this block
   if (t0 >= T) return;
-  int* s_ids = s_buf;
   int* s_dest = s_buf + kChunkTokens * K;
-  const int64_t fc = (int64_t)c * kChunkTokens * K;  // first flat index of the chunk
-  const int base = sub * kSubTokens * K;             // entries of the chunk that precede this block
-  const int n_mine = (int)min((int64_t)kSubTokens * K, (int64_t)T * K - (fc + base));
-  const int n_load = base + n_mine;
-
-  for (int j = threadIdx.x; j < n_load; j += blockDim.x) s_ids[j] = ids[fc + j];
-  __syncthreads();
-  for (int j = threadIdx.x; j < n_mine; j += blockDim.x) {
-    const int e = s_ids[base + j];
-    int rank = 0;
-    for (int i = 0; i < base + j; ++i) rank += (s_ids[i] == e);
-    const int dest = (e >= 0 && e < E) ? expert_start[e] + counts[(size_t)c * E + e] + rank : -1;
-    s_dest[j] = dest;
-    row_id_map[fc + base + j] = dest;
-    if (sorted_indices && dest >= 0) sorted_indices[dest] = fc + base + j;
-  }
-  __syncthreads();
+  scatter_index(ids, T, K, E, c, sub, counts, expert_start, s_buf, s_dest, row_id_map, sorted_indices);
 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
   const int t_in_block = min(kSubTokens, T - t0);
@@ -109,7 +117,7 @@ __global__ void __launch_bounds__(128) permute_scatter_kernel(const uint4* __res
 }
 
 // ---- kernel B', rows moved by the bulk-copy engine (TMA, cp.async.bulk: SASS UBLKCP) ---------------------------------
-// Same index work as permute_scatter_kernel; the token rows never pass through registers: thread 0 stages the block's
+// Same index work as permute_scatter_kernel (scatter_index); the token rows never pass through registers: thread 0 stages the block's
 // kSubTokens rows in shared memory with one bulk load each (issued BEFORE the index work, which they overlap) and, as
 // each row lands (mbarrier complete_tx), one lane fans it out to its K destinations with bulk stores.
 __device__ __forceinline__ uint32_t pm_smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -145,22 +153,7 @@ __global__ void __launch_bounds__(128) permute_scatter_bulk_kernel(const uint8_t
                    : "memory");
     }
   }
-  const int64_t fc = (int64_t)c * kChunkTokens * K;
-  const int base = sub * kSubTokens * K;
-  const int n_mine = (int)min((int64_t)kSubTokens * K, (int64_t)T * K - (fc + base));
-  const int n_load = base + n_mine;
-  for (int j = threadIdx.x; j < n_load; j += blockDim.x) s_ids[j] = ids[fc + j];
-  __syncthreads();
-  for (int j = threadIdx.x; j < n_mine; j += blockDim.x) {
-    const int e = s_ids[base + j];
-    int rank = 0;
-    for (int i = 0; i < base + j; ++i) rank += (s_ids[i] == e);
-    const int dest = (e >= 0 && e < E) ? expert_start[e] + counts[(size_t)c * E + e] + rank : -1;
-    s_dest[j] = dest;
-    row_id_map[fc + base + j] = dest;
-    if (sorted_indices && dest >= 0) sorted_indices[dest] = fc + base + j;
-  }
-  __syncthreads();
+  scatter_index(ids, T, K, E, c, sub, counts, expert_start, s_ids, s_dest, row_id_map, sorted_indices);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
   if (lane == 0) {
     for (int tt = warp; tt < t_in_block; tt += n_warps) {
@@ -190,12 +183,8 @@ __device__ __forceinline__ uint4 combine_epilogue(const float (&acc)[8], const u
 #pragma unroll
   for (int j = 0; j < 8; ++j) c[j] = acc[j];
   if (residual != nullptr) {
-    const uint4 rv = ld_stream_16(residual + vec_index);
     float r[8];
-    unpack_bf16x2(rv.x, r[0], r[1]);
-    unpack_bf16x2(rv.y, r[2], r[3]);
-    unpack_bf16x2(rv.z, r[4], r[5]);
-    unpack_bf16x2(rv.w, r[6], r[7]);
+    unpack_bf16x8(ld_stream_16(residual + vec_index), r);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       float v = rbf(c[j]);
@@ -206,12 +195,7 @@ __device__ __forceinline__ uint4 combine_epilogue(const float (&acc)[8], const u
 #pragma unroll
     for (int j = 0; j < 8; ++j) c[j] = rbf(c[j]) * hidden_factor;
   }
-  uint4 o;
-  o.x = pack_bf16x2(c[0], c[1]);
-  o.y = pack_bf16x2(c[2], c[3]);
-  o.z = pack_bf16x2(c[4], c[5]);
-  o.w = pack_bf16x2(c[6], c[7]);
-  return o;
+  return pack_bf16x8(c);
 }
 
 // ---- a5 unpermute (combine): one warp per token -----------------------------------------------------
@@ -254,10 +238,7 @@ __global__ void __launch_bounds__(256) unpermute_kernel(const uint4* __restrict_
 #pragma unroll
         for (int k = 0; k < KT; ++k) {
           float f[8];
-          unpack_bf16x2(in[u][k].x, f[0], f[1]);
-          unpack_bf16x2(in[u][k].y, f[2], f[3]);
-          unpack_bf16x2(in[u][k].z, f[4], f[5]);
-          unpack_bf16x2(in[u][k].w, f[6], f[7]);
+          unpack_bf16x8(in[u][k], f);
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             // products are rounded before the add, as in `(tokens * probs).sum(dim=1)` of the reference
@@ -277,10 +258,7 @@ __global__ void __launch_bounds__(256) unpermute_kernel(const uint4* __restrict_
         const float pk = probs ? probs[(size_t)t * K + k] : 1.f;
         const uint4 in = ld_stream_16(y + (size_t)r * row_vec + v);
         float f[8];
-        unpack_bf16x2(in.x, f[0], f[1]);
-        unpack_bf16x2(in.y, f[2], f[3]);
-        unpack_bf16x2(in.z, f[4], f[5]);
-        unpack_bf16x2(in.w, f[6], f[7]);
+        unpack_bf16x8(in, f);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float prod = probs ? __fmul_rn(f[j], pk) : f[j];
@@ -323,10 +301,7 @@ __global__ void __launch_bounds__(256) unpermute_bwd_kernel(const uint4* __restr
           const int v = v0 + u * 32;
           if (v >= row_vec) continue;
           float gf[8];
-          unpack_bf16x2(g[u].x, gf[0], gf[1]);
-          unpack_bf16x2(g[u].y, gf[2], gf[3]);
-          unpack_bf16x2(g[u].z, gf[4], gf[5]);
-          unpack_bf16x2(g[u].w, gf[6], gf[7]);
+          unpack_bf16x8(g[u], gf);
           uint4 o;
           o.x = pack_bf16x2(gf[0] * pk, gf[1] * pk);
           o.y = pack_bf16x2(gf[2] * pk, gf[3] * pk);
@@ -335,10 +310,7 @@ __global__ void __launch_bounds__(256) unpermute_bwd_kernel(const uint4* __restr
           st_stream_16(act_grad + (size_t)r * row_vec + v, o);
           if (prob_grad) {
             float yf[8];
-            unpack_bf16x2(yv[u].x, yf[0], yf[1]);
-            unpack_bf16x2(yv[u].y, yf[2], yf[3]);
-            unpack_bf16x2(yv[u].z, yf[4], yf[5]);
-            unpack_bf16x2(yv[u].w, yf[6], yf[7]);
+            unpack_bf16x8(yv[u], yf);
 #pragma unroll
             for (int j = 0; j < 8; ++j) dot = fmaf(gf[j], yf[j], dot);
           }
