@@ -222,11 +222,13 @@ int xtb_lm_head_ce(const void* h, const void* w, const int64_t* labels, const fl
                    int64_t ignore_index, int need_grad, void* z_or_G, void* workspace, float* row_ce, float* loss, void* dh,
                    void* dW, xtb_stream_t stream);
 /* ---- a8  native_swiglu: ops/act_fn.py:7-9 ---------------------------------------------------------
- * out[m, j] = bf16( bf16(silu(h[m, j])) * h[m, I + j] ),  h is [M, 2I] bf16 (gate | up). */
+ * out[m, j] = bf16( bf16(silu(h[m, j])) * h[m, I + j] ),  h is [M, 2I] bf16 (gate | up).  I % 8 == 0; every pointer of
+ * both entries 16-byte aligned. */
 int xtb_swiglu(const void* h_bf16, void* out_bf16, int64_t M, int I, xtb_stream_t stream);
 /* autograd of the two eager ops (silu, mul) with their bf16 roundings:
  *   grad_h[m, I + j] = bf16(g * s),  s = bf16(silu(x1));  d_s = bf16(g * x2);
- *   grad_h[m, j]     = bf16( d_s * sigmoid(x1) * (1 + x1 * (1 - sigmoid(x1))) ) */
+ *   grad_h[m, j]     = bf16( d_s * sigmoid(x1) * (1 + x1 * (1 - sigmoid(x1))) )
+ * I / 8 <= 23170 (the row split's 32-bit reciprocal). */
 int xtb_swiglu_bwd(const void* grad_out_bf16, const void* h_bf16, void* grad_h_bf16, int64_t M, int I,
                    xtb_stream_t stream);
 
@@ -282,8 +284,11 @@ int xtb_qk_norm_rope_bwd(const void* g_q_bf16, int64_t g_q_stride_t, int64_t g_q
 
 /* ==== fp8 tile-wise quantisation (row a15, config 5) ============================================================
  * e4m3, scale = clamp(amax, 1e-12) / 448 (xtuner/v1/float8/float8_utils.py:6-32, fsdp_utils.py:75-116,195-223,
- * triton_kernels/per_tile_quant.py:61-100).  Bit-exact against reference-made golden vectors on an H100
- * (tests/test_gpu_fp8.py).  Nothing on the bf16 default path calls these; `plugin.install_fp8_cast()` rebinds the
+ * triton_kernels/per_tile_quant.py:61-100).  Bit-exact on an H100 against reference-made golden vectors
+ * (tests/test_gpu_fp8.py), and against the oracle and the reference's own functions on every bf16 value in
+ * [-448, 448], all-zero blocks, fp32 and bf16 weights and NaN / inf inputs (tests/test_gpu_fp8_edges.py): a NaN makes
+ * its tile's or block's scale and bytes NaN, an inf gives an inf scale.  x must be 8-byte aligned, q and scales 4-byte
+ * aligned; nw <= 65535.  Nothing on the bf16 default path calls these; `plugin.install_fp8_cast()` rebinds the
  * reference's FSDP fp8 all-gather cast (`WeightWithDynamicTilewiseFloat8CastTensor.fsdp_pre_all_gather`,
  * fsdp_utils.py:379-409) and its scale precompute to them.  There is no fp8 grouped GEMM here yet. */
 int xtb_fp8_per_tile_quant(const void* x_bf16, void* q_e4m3, float* scales /*[M, K/128]*/, int64_t M, int64_t K,

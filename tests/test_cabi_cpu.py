@@ -60,6 +60,23 @@ def test_argument_validation_is_host_side(lib):
     assert lib.xtb_moe_permute_workspace_bytes(8192, 2, 8) > 0
 
 
+def test_swiglu_and_fp8_alignment_and_grid_limits_are_host_side(lib):
+    """The SwiGLU kernels move 16-byte vectors, the fp8 tile kernel 8-byte loads and 4-byte stores, and the fp8 block
+    kernels put one matrix per grid z index: a pointer or count they cannot take is refused before any CUDA call.  The
+    pointer values are never dereferenced."""
+    A = 1 << 20  # a 16-byte aligned fake address
+    for args in ((A + 8, A), (A, A + 2)):
+        assert lib.xtb_swiglu(*args, 4, 64, None) == 1 and b"16-byte aligned" in lib.xtb_last_error()
+    for args in ((A + 8, A, A), (A, A + 4, A), (A, A, A + 2)):
+        assert lib.xtb_swiglu_bwd(*args, 4, 64, None) == 1 and b"16-byte aligned" in lib.xtb_last_error()
+    for args in ((A + 4, A, A), (A, A + 2, A), (A, A, A + 2)):
+        assert lib.xtb_fp8_per_tile_quant(*args, 4, 128, None) == 1 and b"aligned" in lib.xtb_last_error()
+    assert lib.xtb_fp8_block_scales(A, 1, 65536, 128, 128, A, None) == 1 and b"65535" in lib.xtb_last_error()
+    assert lib.xtb_fp8_block_cast(A, 0, 65536, 128, 128, A, A, None) == 1 and b"65535" in lib.xtb_last_error()
+    # the widest SwiGLU backward row the 32-bit reciprocal row split takes is I = 8 * 23170
+    assert lib.xtb_swiglu_bwd(A, A, A, 4, 8 * 23171, None) == 1 and b"too wide" in lib.xtb_last_error()
+
+
 def test_every_compute_entry_rejects_null_pointers_on_the_host(lib):
     """Error behaviour of the boundary: a bad call returns XTB_ERR_INVALID (1) with a message naming the entry point —
     before any CUDA call, so it holds without a GPU — instead of crashing."""

@@ -1,6 +1,9 @@
 // fp8 (e4m3) tile-wise quantisation kernels for the fp8 expert path (SURVEY.md §8a row a15, config 5).
 // Bit-exact on an H100 against reference-made golden vectors and the oracle (tests/test_gpu_fp8.py; oracle/moe_oracle.py:
-// per_tile_quant, per_block_fp8_scales, cast_to_per_block_fp8).  Nothing on the bf16 default path calls them;
+// per_tile_quant, per_block_fp8_scales, cast_to_per_block_fp8), and against the reference's own functions on CUDA tensors
+// (tests/test_gpu_fp8_edges.py): every bf16 value in [-448, 448] through the cast, all-zero and sub-1e-12 blocks, fp32 and
+// bf16 weights, and NaN / inf inputs, where the scale follows torch's amax (a NaN makes its whole tile or block NaN, an
+// inf gives an inf scale and inf / inf = NaN).  Nothing on the bf16 default path calls them;
 // plugin.install_fp8_cast() rebinds the reference's fp8 FSDP all-gather cast and scale precompute to them.
 //
 //   xtb_fp8_per_tile_quant   activations [M,K] bf16 -> e4m3 [M,K] + fp32 scale per 1x128 tile
@@ -9,20 +12,29 @@
 //                            (float8/fsdp_utils.py:75-116, dout >= 128 branch)
 //   xtb_fp8_block_cast       weights [dout,din] + scales -> e4m3 [dout,din]   (float8/fsdp_utils.py:195-223)
 // scale = clamp(amax, 1e-12) / 448 evaluated in double like the reference (fsdp_utils.py:106-110), value / scale in
-// fp32, saturating round-to-nearest-even conversion (float8_utils.py:16-32).
+// fp32, saturating round-to-nearest-even conversion (float8_utils.py:16-32; NaN stays NaN, +-inf and finite overflow
+// become +-448).
 #include <cuda_fp8.h>
 
 #include "common.cuh"
 
 namespace xtb {
 
+// max that keeps NaN, as torch's amax does (fmaxf drops a NaN operand, which would leave the scale finite)
+__device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
+__device__ __forceinline__ float warp_nan_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = nan_max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
 __device__ __forceinline__ float fp8_scale_from_amax(float amax) {
   const double a = amax < 1e-12 ? 1e-12 : (double)amax;
   return (float)(a / 448.0);
 }
 
+// satfinite: finite overflow and +-inf saturate to +-448 (the reference's clamp), NaN converts to NaN
 __device__ __forceinline__ uint8_t to_e4m3_sat(float v) {
-  v = fminf(fmaxf(v, -448.f), 448.f);
   return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3);
 }
 
@@ -37,8 +49,8 @@ __global__ void __launch_bounds__(256) fp8_per_tile_quant_kernel(const __nv_bflo
   float f[4];
   unpack_bf16x2(raw.x, f[0], f[1]);
   unpack_bf16x2(raw.y, f[2], f[3]);
-  float amax = fmaxf(fmaxf(fabsf(f[0]), fabsf(f[1])), fmaxf(fabsf(f[2]), fabsf(f[3])));
-  amax = warp_max(amax);
+  float amax = nan_max(nan_max(fabsf(f[0]), fabsf(f[1])), nan_max(fabsf(f[2]), fabsf(f[3])));
+  amax = warp_nan_max(amax);
   const float s = fp8_scale_from_amax(amax);
   if (lane == 0) scales[tile] = s;
   uint32_t out = 0;
@@ -65,14 +77,14 @@ __global__ void __launch_bounds__(256) fp8_block_kernel(const T* __restrict__ w,
       float v;
       if constexpr (sizeof(T) == 2) v = __bfloat162float(base[(long long)r * din + c]);
       else v = (float)base[(long long)r * din + c];
-      amax = fmaxf(amax, fabsf(v));
+      amax = nan_max(amax, fabsf(v));
     }
-    amax = warp_max(amax);
+    amax = warp_nan_max(amax);
     if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = amax;
     __syncthreads();
     if (threadIdx.x == 0) {
       float m = s_red[0];
-      for (int i = 1; i < 8; ++i) m = fmaxf(m, s_red[i]);
+      for (int i = 1; i < 8; ++i) m = nan_max(m, s_red[i]);
       scales_out[(mat * nbi + bi) * nbj + bj] = fp8_scale_from_amax(m);
     }
     return;
@@ -97,6 +109,10 @@ extern "C" int xtb_fp8_per_tile_quant(const void* x_bf16, void* q_e4m3, float* s
                                       xtb_stream_t stream) {
   XTB_CHECK_ARG(x_bf16 && q_e4m3 && scales, "xtb_fp8_per_tile_quant: null pointer");
   XTB_CHECK_ARG(M >= 0 && K > 0 && K % 128 == 0, "xtb_fp8_per_tile_quant: K=%lld must be a multiple of 128", (long long)K);
+  // 8-byte loads of x, 4-byte stores of q
+  XTB_CHECK_ARG(reinterpret_cast<uintptr_t>(x_bf16) % 8 == 0 && reinterpret_cast<uintptr_t>(q_e4m3) % 4 == 0 &&
+                    reinterpret_cast<uintptr_t>(scales) % 4 == 0,
+                "xtb_fp8_per_tile_quant: x must be 8-byte aligned, q and scales 4-byte aligned");
   XTB_ENSURE_CTX(x_bf16);
   const long long n_tiles = M * (K / 128);
   if (n_tiles == 0) return XTB_OK;
@@ -111,6 +127,7 @@ extern "C" int xtb_fp8_block_scales(const void* w, int w_is_f32, int64_t nw, int
   XTB_CHECK_ARG(w && scales, "xtb_fp8_block_scales: null pointer");
   XTB_CHECK_ARG(nw >= 0 && dout > 0 && din > 0 && dout % 128 == 0 && din % 128 == 0,
                 "xtb_fp8_block_scales: dout=%d, din=%d must be multiples of 128", dout, din);
+  XTB_CHECK_ARG(nw <= 65535, "xtb_fp8_block_scales: nw=%lld exceeds the grid's z limit 65535", (long long)nw);
   XTB_ENSURE_CTX(w);
   if (nw == 0) return XTB_OK;
   dim3 grid(din / 128, dout / 128, (unsigned)nw);
@@ -125,6 +142,7 @@ extern "C" int xtb_fp8_block_cast(const void* w, int w_is_f32, int64_t nw, int d
   XTB_CHECK_ARG(w && scales && q_e4m3, "xtb_fp8_block_cast: null pointer");
   XTB_CHECK_ARG(nw >= 0 && dout > 0 && din > 0 && dout % 128 == 0 && din % 128 == 0,
                 "xtb_fp8_block_cast: dout=%d, din=%d must be multiples of 128", dout, din);
+  XTB_CHECK_ARG(nw <= 65535, "xtb_fp8_block_cast: nw=%lld exceeds the grid's z limit 65535", (long long)nw);
   XTB_ENSURE_CTX(w);
   if (nw == 0) return XTB_OK;
   dim3 grid(din / 128, dout / 128, (unsigned)nw);

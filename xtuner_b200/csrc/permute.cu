@@ -552,6 +552,8 @@ extern "C" int xtb_moe_unpermute_bwd(const void* grad_out_bf16, const void* y_fw
 extern "C" int xtb_swiglu(const void* h_bf16, void* out_bf16, int64_t M, int I, xtb_stream_t stream) {
   XTB_CHECK_ARG(h_bf16 && out_bf16, "xtb_swiglu: null pointer");
   XTB_CHECK_ARG(M >= 0 && I > 0 && I % 8 == 0, "xtb_swiglu: bad M=%lld I=%d (I%%8==0)", (long long)M, I);
+  XTB_CHECK_ARG((reinterpret_cast<uintptr_t>(h_bf16) | reinterpret_cast<uintptr_t>(out_bf16)) % 16 == 0,
+                "xtb_swiglu: pointers must be 16-byte aligned");
   XTB_ENSURE_CTX(h_bf16);
   if (M == 0) return XTB_OK;
   const int64_t n = M * (I / 8);
@@ -565,12 +567,15 @@ extern "C" int xtb_swiglu_bwd(const void* grad_out_bf16, const void* h_bf16, voi
                               xtb_stream_t stream) {
   XTB_CHECK_ARG(grad_out_bf16 && h_bf16 && grad_h_bf16, "xtb_swiglu_bwd: null pointer");
   XTB_CHECK_ARG(M >= 0 && I > 0 && I % 8 == 0, "xtb_swiglu_bwd: bad shape");
-  XTB_ENSURE_CTX(h_bf16);
-  if (M == 0) return XTB_OK;
+  XTB_CHECK_ARG((reinterpret_cast<uintptr_t>(grad_out_bf16) | reinterpret_cast<uintptr_t>(h_bf16) |
+                 reinterpret_cast<uintptr_t>(grad_h_bf16)) % 16 == 0,
+                "xtb_swiglu_bwd: pointers must be 16-byte aligned");
   const int64_t n = M * (I / 8);
   const int I8 = I / 8;
   // floor(i / I8) == umulhi(i, ceil(2^32 / I8)) as long as i * I8 < 2^32; i < kSwRows * I8 inside a block
   XTB_CHECK_ARG((int64_t)kSwRows * I8 * I8 < (1ll << 32), "xtb_swiglu_bwd: I=%d too wide", I);
+  XTB_ENSURE_CTX(h_bf16);
+  if (M == 0) return XTB_OK;
   const uint32_t inv_I8 = (uint32_t)(((1ull << 32) + I8 - 1) / I8);
   (void)n;
   XTB_CUDA(launch_pdl(swiglu_bwd_kernel, dim3((unsigned)((M + kSwRows - 1) / kSwRows)), dim3(256), 0, as_stream(stream), 
