@@ -92,6 +92,40 @@ int xtb_gate_route_dispatch(const void* x_bf16, const float* w_f32, int T, int H
                             int norm_topk_prob, float scaling, float* logits, float* router_weights,
                             float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32, int64_t* tokens_per_expert,
                             void* dispatch_workspace, xtb_stream_t stream);
+/* ---- routing replay (RL rollout-routed experts) --------------------------------------------------------
+ * The reference's RL trainer feeds back the experts the rollout engine chose, seq_ctx.rollout_routed_experts, an int64
+ * [S, L, K] tensor (rl/trainer/worker.py:476-550); each decoder layer hands its slice [:, layer_idx, :] to the router
+ * (moe_decoder_layer.py:669-678), which then gathers its weights at those ids instead of taking a top-k
+ * (router/greedy.py:74-78, router/noaux_router.py:114-121).  The replay entries below take those ids as
+ * replay_ids[t * replay_row_stride + k] (k < K, replay_row_stride >= K elements, column stride 1), so the layer slice of
+ * the [S, L, K] tensor is passed without a copy.  They produce every output of their routing counterpart, computed
+ * with the same per-token code (csrc/greedy_router.cuh): the scores are the same bits, and replaying the ids the
+ * routing entry chose reproduces all of its outputs, the dispatch workspace included, bit for bit.
+ *   The ids come from outside the program (rollout workers, through ray), so they are checked, never trusted:
+ *   - an id outside [0, E) is written as 0 to topk_ids and topk_ids_i32, every topk weight of its token is NaN, and
+ *     the slot is counted under expert 0 in tokens_per_expert and in the dispatch workspace.  Permute, the grouped GEMMs,
+ *     combine and every backward entry therefore stay in bounds; the token's layer output rows are NaN, the step's loss
+ *     is non-finite, and the reference trainer skips a step whose gradient norm is not finite
+ *     (engine/train_engine.py:312);
+ *   - duplicate ids in a row are valid (the reference's own padding ids are randint draws,
+ *     rl/trainer/controller.py:150-152): they are gathered, counted and dispatched twice, as in the reference.
+ * No new backward: xtb_router_greedy_bwd, xtb_router_gate_bwd and xtb_router_noaux_bwd read topk_ids and add each
+ * slot's contribution (gather's backward, a scatter-add), which holds for replayed ids, duplicates included. */
+/* a2 with replayed ids: the outputs of xtb_router_greedy; with dispatch_workspace (nullable) also fills it exactly as
+ * xtb_router_greedy_dispatch does (topk_ids_i32 then required).  E <= 512, K <= 8. */
+int xtb_router_greedy_replay(const float* logits, const int64_t* replay_ids, int64_t replay_row_stride, int T, int E,
+                             int K, int scoring, int norm_topk_prob, float scaling, float* router_weights,
+                             float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32, int64_t* tokens_per_expert,
+                             void* dispatch_workspace, xtb_stream_t stream);
+/* xtb_gate_route_dispatch with replayed ids: gate on the tensor cores, then the per-token replay of
+ * xtb_router_greedy_replay and the dispatch bucketing in one launch.  Same limits: E <= 8, K <= 8, H % 128 == 0,
+ * H <= 4224; XTB_ERR_INVALID otherwise (use xtb_gate_logits + xtb_router_greedy_replay). */
+int xtb_gate_route_replay_dispatch(const void* x_bf16, const float* w_f32, const int64_t* replay_ids,
+                                   int64_t replay_row_stride, int T, int H, int E, int K, int scoring,
+                                   int norm_topk_prob, float scaling, float* logits, float* router_weights,
+                                   float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32,
+                                   int64_t* tokens_per_expert, void* dispatch_workspace, xtb_stream_t stream);
+
 /* backward of a2 through its three differentiable outputs (SURVEY.md Appendix B "three routes"):
  * grad_logits[T,E] = d(topk_weights)·grad_topk_weights + d(router_weights)·grad_router_weights
  *                    (+ grad_logits_direct if not NULL).  Either grad input may be NULL (treated as 0). */
@@ -120,6 +154,16 @@ int xtb_router_noaux(const float* logits, const float* e_score_correction_bias, 
                      int topk_group, int norm_topk_prob, float scaling, float* router_weights,
                      float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32, float* tokens_per_expert_f32,
                      xtb_stream_t stream);
+
+/* a2' with replayed ids (see "routing replay" above): router_weights and tokens_per_expert_f32 as xtb_router_noaux —
+ * the reference's router_weights do not depend on the replayed ids; topk weights = the unbiased sigmoid at the given ids,
+ * renormalised with +1e-20 when K > 1 and norm_topk_prob, then scaled.  The top-k the reference computes and discards is
+ * skipped.  Same E / n_group limits as xtb_router_noaux. */
+int xtb_router_noaux_replay(const float* logits, const float* e_score_correction_bias, const int64_t* replay_ids,
+                            int64_t replay_row_stride, int T, int E, int K, int n_group, int topk_group,
+                            int norm_topk_prob, float scaling, float* router_weights, float* topk_weights,
+                            int64_t* topk_ids, int32_t* topk_ids_i32, float* tokens_per_expert_f32,
+                            xtb_stream_t stream);
 
 /* backward of a2' (what autograd does to noaux_router.py:80-134; closed form in oracle/moe_oracle.py
  * noaux_router_bwd).  Inputs are the forward's inputs and outputs, and its group geometry as

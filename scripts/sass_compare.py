@@ -23,7 +23,8 @@ def dropped(d):  # a template parameter removed together with its other value: <
 same=diff=0
 for k,v in old.items():
     d=demangle(k)
-    cands=[nk for nd,nk in newd.items() if nd in (d, dropped(d)) or nd.replace(", false>",">")==d or nd.replace(", (bool)0>",">")==d]
+    cands=[nk for nd,nk in newd.items() if nd in (d, dropped(d)) or nd.replace(", false>",">")==d or nd.replace(", (bool)0>",">")==d
+           or re.sub(r"^void (\S+)<false>$", r"\1", nd)==d]  # a kernel that became a template over an off-by-default switch
     if not cands:
         print("MISSING in new:", d); continue
     nv=new[cands[0]]

@@ -45,6 +45,21 @@ SIGNATURES = {
         [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
          c_void_p, c_void_p, c_void_p],
     ),
+    "xtb_router_greedy_replay": (
+        c_int,
+        [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+         c_void_p, c_void_p, c_void_p],
+    ),
+    "xtb_gate_route_replay_dispatch": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
+         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
+    "xtb_router_noaux_replay": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
+         c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
     "xtb_router_greedy_bwd": (
         c_int,
         [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p],

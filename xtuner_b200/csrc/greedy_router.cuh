@@ -1,6 +1,6 @@
-// The greedy router's per-token arithmetic, forward and backward.  The standalone router kernels (route.cu) and the fused
-// gate + route (gate_mma.cu) and router + gate backward (route.cu) kernels all call these bodies, so they route and
-// differentiate every token the same way, bit for bit.
+// The greedy router's per-token arithmetic, forward, routing replay and backward.  The standalone router kernels
+// (route.cu) and the fused gate + route (gate_mma.cuh) and router + gate backward (route.cu) kernels all call these
+// bodies, so they route and differentiate every token the same way, bit for bit.
 //
 // LPT lanes cooperate on one token; each lane holds VPL consecutive experts e = e0 + j (e0 = lane-in-group * VPL).
 // With LPT = 1 every shuffle loop below is empty and one thread routes its token alone.
@@ -87,6 +87,50 @@ __device__ __forceinline__ void greedy_route_token(const float* lg, int e0, int 
       if (norm_topk) wv = wv / sum;
       if (scaling != 1.0f) wv = wv * scaling;
       sel_w[k] = wv;
+    }
+  }
+}
+
+// Routing replay (greedy.py:74-78, `routing_weights.gather(dim=1, index=rollout_routed_experts)`): the experts are the
+// K given ids ids[0, K) instead of a top-k.  The scores are greedy_route_token's own code with K = 0 (no selection), so
+// they are the same bits as routing; each weight is gathered across the group with the reduction greedy_route_token_bwd
+// uses (the one lane holding the expert contributes p, the others 0), then the weights are summed in k order and
+// renormalised and scaled as in greedy_route_token.  The ids come from outside the program (rollout workers), so they
+// are checked, never trusted: an id outside [0, E) becomes expert 0 in sel_e and makes every weight of the token NaN.
+// Duplicate ids are gathered twice, as gather does.  Out: as greedy_route_token.
+template <int LPT, int VPL>
+__device__ __forceinline__ void greedy_replay_token(const float* lg, const int64_t* __restrict__ ids, int e0, int E,
+                                                    int K, int scoring, int norm_topk, float scaling, float (&p)[VPL],
+                                                    float (&sel_w)[8], int (&sel_e)[8]) {
+  greedy_route_token<LPT, VPL>(lg, e0, E, 0, scoring, norm_topk, scaling, p, sel_w, sel_e);
+  float sum = 0.f;
+  bool bad = false;
+  // unrolled, so that sel_w / sel_e stay in registers
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    if (k < K) {
+      const int64_t raw = ids[k];
+      const bool ok = raw >= 0 && raw < E;
+      const int id = ok ? (int)raw : 0;
+      float v = 0.f;
+#pragma unroll
+      for (int j = 0; j < VPL; ++j)
+        if (e0 + j == id) v = p[j];
+#pragma unroll
+      for (int o = LPT / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      bad |= !ok;
+      sel_w[k] = v;
+      sel_e[k] = id;
+      sum += v;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    if (k < K) {
+      float wv = sel_w[k];
+      if (norm_topk) wv = wv / sum;
+      if (scaling != 1.0f) wv = wv * scaling;
+      sel_w[k] = bad ? __int_as_float(0x7fffffff) : wv;  // NaN
     }
   }
 }

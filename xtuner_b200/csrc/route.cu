@@ -301,17 +301,19 @@ __global__ void colsum_kernel(const float* __restrict__ gl, float* __restrict__ 
 // =====================================================================================================
 // a2  greedy router.  LPT lanes cooperate on one token; each lane holds VPL consecutive experts
 // (e = sub*VPL + j); the per-token arithmetic is greedy_route_token (greedy_router.cuh).  Histogram:
-// warp-aggregated shared-memory counters, one global atomic per (block, expert).
+// warp-aggregated shared-memory counters, one global atomic per (block, expert).  REPLAY: the experts are the
+// rows of replay_ids (row stride replay_stride elements) instead of a top-k (greedy_replay_token).
 // =====================================================================================================
-template <int LPT, int VPL>
-__global__ void __launch_bounds__((LPT * 32 > 256) ? LPT * 32 : 256)
+// (REPLAY asks for one resident block per SM: left to itself, ptxas gives <32, 8, true> 32 registers and a spill)
+template <int LPT, int VPL, bool REPLAY = false>
+__global__ void __launch_bounds__((LPT * 32 > 256) ? LPT * 32 : 256, REPLAY ? 1 : 0)
 router_greedy_kernel(const float* __restrict__ logits, int T, int E, int K, int scoring, int norm_topk, float scaling,
                      float* __restrict__ router_weights, float* __restrict__ topk_weights,
                      int64_t* __restrict__ topk_ids, int32_t* __restrict__ topk_ids_i32,
                      unsigned long long* __restrict__ tokens_per_expert,
                      // optional: prepare the dispatch workspace (per-chunk histograms + scan) in this launch
                      int* __restrict__ chunk_counts, int* __restrict__ expert_start, unsigned* __restrict__ ticket,
-                     int n_chunks) {
+                     int n_chunks, const int64_t* __restrict__ replay_ids = nullptr, int64_t replay_stride = 0) {
   pdl_sync();
   // blockDim.x / LPT tokens per block, always a multiple of kChunkTokens (= 32)
   extern __shared__ int s_hist[];  // [E] block histogram | [chunks_per_block][E] per-chunk histograms
@@ -329,7 +331,11 @@ router_greedy_kernel(const float* __restrict__ logits, int T, int E, int K, int 
 
   float p[VPL], sel_w[8];
   int sel_e[8];
-  greedy_route_token<LPT, VPL>(logits + (size_t)tok * E, e0, E, K, scoring, norm_topk, scaling, p, sel_w, sel_e);
+  if constexpr (REPLAY)
+    greedy_replay_token<LPT, VPL>(logits + (size_t)tok * E, replay_ids + tok * replay_stride, e0, E, K, scoring,
+                                  norm_topk, scaling, p, sel_w, sel_e);
+  else
+    greedy_route_token<LPT, VPL>(logits + (size_t)tok * E, e0, E, K, scoring, norm_topk, scaling, p, sel_w, sel_e);
   if (active) {
 #pragma unroll
     for (int j = 0; j < VPL; ++j)
@@ -387,7 +393,11 @@ __global__ void __launch_bounds__(256) router_greedy_bwd_kernel(
 // =====================================================================================================
 // a2' no-aux router: one warp per token, lane holds VPL = E/32 consecutive experts.
 // =====================================================================================================
-template <int VPL>
+// REPLAY (noaux_router.py:114-121): router_weights as above — they do not depend on the ids — and the topk weights
+// gathered from the unbiased scores at the rows of replay_ids (row stride replay_stride elements) in place of the
+// top-k, which the reference computes and discards.  An id outside [0, E) becomes expert 0 and makes every topk weight
+// of its token NaN.
+template <int VPL, bool REPLAY = false>
 __global__ void __launch_bounds__(256) router_noaux_kernel(const float* __restrict__ logits,
                                                            const float* __restrict__ bias, int T, int E, int K,
                                                            int n_group, int topk_group, int norm_topk,
@@ -395,7 +405,10 @@ __global__ void __launch_bounds__(256) router_noaux_kernel(const float* __restri
                                                            float* __restrict__ topk_weights,
                                                            int64_t* __restrict__ topk_ids,
                                                            int32_t* __restrict__ topk_ids_i32,
-                                                           float* __restrict__ tokens_per_expert) {
+                                                           float* __restrict__ tokens_per_expert,
+                                                           const int64_t* __restrict__ replay_ids = nullptr,
+                                                           int64_t replay_stride = 0) {
+  if constexpr (REPLAY) pdl_sync();
   extern __shared__ int s_hist[];
   for (int i = threadIdx.x; i < E; i += blockDim.x) s_hist[i] = 0;
   __syncthreads();
@@ -465,35 +478,54 @@ __global__ void __launch_bounds__(256) router_noaux_kernel(const float* __restri
     for (int j = 0; j < VPL; ++j) router_weights[(size_t)token * E + e0 + j] = ch[j] / rs;
   }
   // top-k over the (masked) choice scores, weights from the unbiased scores
-  unsigned taken = 0;
   float sel_w[32];
   int sel_e[32];
   float sum = 0.f;
-  for (int k = 0; k < K; ++k) {
-    float bv = -INFINITY, bw = 0.f;
-    int be = 0x7fffffff;
+  bool bad = false;
+  if constexpr (REPLAY) {
+    const int64_t* ids = replay_ids + tok * replay_stride;
+    for (int k = 0; k < K; ++k) {
+      const int64_t raw = ids[k];
+      const bool ok = raw >= 0 && raw < E;
+      const int id = ok ? (int)raw : 0;
+      float bw = 0.f;
 #pragma unroll
-    for (int j = 0; j < VPL; ++j) {
-      if (!((taken >> j) & 1u) && ch[j] > bv) { bv = ch[j]; be = e0 + j; bw = sc[j]; }
+      for (int j = 0; j < VPL; ++j)
+        if (e0 + j == id) bw = sc[j];
+      bw = warp_sum(bw);  // one lane holds expert id; the others add 0
+      bad |= !ok;
+      sel_w[k] = bw;
+      sel_e[k] = id;
+      sum += bw;
     }
+  } else {
+    unsigned taken = 0;
+    for (int k = 0; k < K; ++k) {
+      float bv = -INFINITY, bw = 0.f;
+      int be = 0x7fffffff;
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      const int oe = __shfl_xor_sync(0xffffffffu, be, o);
-      const float ow = __shfl_xor_sync(0xffffffffu, bw, o);
-      if (ov > bv || (ov == bv && oe < be)) { bv = ov; be = oe; bw = ow; }
+      for (int j = 0; j < VPL; ++j) {
+        if (!((taken >> j) & 1u) && ch[j] > bv) { bv = ch[j]; be = e0 + j; bw = sc[j]; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oe = __shfl_xor_sync(0xffffffffu, be, o);
+        const float ow = __shfl_xor_sync(0xffffffffu, bw, o);
+        if (ov > bv || (ov == bv && oe < be)) { bv = ov; be = oe; bw = ow; }
+      }
+      if (be < 0 || be >= E) {  // no score left that compares (NaN or -inf): the lowest index not selected yet, with
+                                // weight 0.  sel_e is the same on every lane, and that index is at most k < K <= E.
+        unsigned used = 0;
+        for (int i = 0; i < k; ++i)
+          if (sel_e[i] < 32) used |= 1u << sel_e[i];
+        be = __ffs(~used) - 1;
+        bw = 0.f;
+      }
+      if (be >= e0 && be < e0 + VPL) taken |= 1u << (be - e0);
+      if (k < 32) { sel_w[k] = bw; sel_e[k] = be; }
+      sum += bw;
     }
-    if (be < 0 || be >= E) {  // no score left that compares (NaN or -inf): the lowest index not selected yet, with
-                              // weight 0.  sel_e is the same on every lane, and that index is at most k < K <= E.
-      unsigned used = 0;
-      for (int i = 0; i < k; ++i)
-        if (sel_e[i] < 32) used |= 1u << sel_e[i];
-      be = __ffs(~used) - 1;
-      bw = 0.f;
-    }
-    if (be >= e0 && be < e0 + VPL) taken |= 1u << (be - e0);
-    if (k < 32) { sel_w[k] = bw; sel_e[k] = be; }
-    sum += bw;
   }
   if (active && lane == 0) {
     const float denom = sum + 1e-20f;
@@ -501,6 +533,7 @@ __global__ void __launch_bounds__(256) router_noaux_kernel(const float* __restri
       float wv = sel_w[k];
       if (K > 1 && norm_topk) wv = wv / denom;
       wv = wv * scaling;
+      if (REPLAY && bad) wv = __int_as_float(0x7fffffff);  // NaN
       topk_weights[(size_t)token * K + k] = wv;
       topk_ids[(size_t)token * K + k] = (int64_t)sel_e[k];
       if (topk_ids_i32) topk_ids_i32[(size_t)token * K + k] = sel_e[k];
@@ -771,7 +804,7 @@ extern "C" int xtb_gate_logits_bwd(const float* grad_logits, const void* x_bf16,
 template <int LPT, int VPL>
 static int launch_router_greedy(const float* logits, int T, int E, int K, int scoring, int norm, float scaling,
                                 float* rw, float* tw, int64_t* ids, int32_t* ids32, int64_t* tpe, void* dispatch_ws,
-                                cudaStream_t st) {
+                                const int64_t* replay_ids, int64_t replay_stride, cudaStream_t st) {
   constexpr int kThreads = (LPT * 32 > 256) ? LPT * 32 : 256;
   const int tokens_per_block = kThreads / LPT;
   const int blocks = (T + tokens_per_block - 1) / tokens_per_block;
@@ -788,9 +821,10 @@ static int launch_router_greedy(const float* logits, int T, int E, int K, int sc
   } else {
     XTB_CUDA(cudaMemsetAsync(tpe, 0, sizeof(int64_t) * E, st));
   }
-  XTB_CUDA(launch_pdl(router_greedy_kernel<LPT, VPL>, dim3(blocks), dim3(kThreads), smem, st, 
-      logits, T, E, K, scoring, norm, scaling, rw, tw, ids, ids32, reinterpret_cast<unsigned long long*>(tpe), counts,
-      estart, ticket, n_chunks_of(T)));
+  XTB_CUDA(launch_pdl(replay_ids ? router_greedy_kernel<LPT, VPL, true> : router_greedy_kernel<LPT, VPL>, dim3(blocks),
+                      dim3(kThreads), smem, st, logits, T, E, K, scoring, norm, scaling, rw, tw, ids, ids32,
+                      reinterpret_cast<unsigned long long*>(tpe), counts, estart, ticket, n_chunks_of(T), replay_ids,
+                      replay_stride));
   XTB_LAUNCH_OK();
   return XTB_OK;
 }
@@ -831,7 +865,8 @@ static int launch_router_noaux_bwd(const float* logits, const float* bias, const
 
 static int router_greedy_impl(const float* logits, int T, int E, int K, int scoring, int norm_topk_prob, float scaling,
                               float* router_weights, float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32,
-                              int64_t* tokens_per_expert, void* dispatch_ws, xtb_stream_t stream) {
+                              int64_t* tokens_per_expert, void* dispatch_ws, xtb_stream_t stream,
+                              const int64_t* replay_ids = nullptr, int64_t replay_stride = 0) {
   XTB_CHECK_ARG(logits && router_weights && topk_weights && topk_ids && tokens_per_expert,
                 "xtb_router_greedy: null pointer");
   XTB_CHECK_ARG(T >= 0 && E > 0 && K > 0 && K <= E && K <= 8, "xtb_router_greedy: bad shape T=%d E=%d K=%d (K<=8)", T,
@@ -843,7 +878,8 @@ static int router_greedy_impl(const float* logits, int T, int E, int K, int scor
     return XTB_OK;
   }
   XTB_ROUTER_DISPATCH(launch_router_greedy, logits, T, E, K, scoring, norm_topk_prob, scaling, router_weights,
-                      topk_weights, topk_ids, topk_ids_i32, tokens_per_expert, dispatch_ws, st)
+                      topk_weights, topk_ids, topk_ids_i32, tokens_per_expert, dispatch_ws, replay_ids, replay_stride,
+                      st)
 }
 
 extern "C" int xtb_router_greedy(const float* logits, int T, int E, int K, int scoring, int norm_topk_prob,
@@ -862,6 +898,25 @@ extern "C" int xtb_router_greedy_dispatch(const float* logits, int T, int E, int
                             topk_ids_i32, tokens_per_expert, dispatch_workspace, stream);
 }
 
+extern "C" int xtb_router_greedy_replay(const float* logits, const int64_t* replay_ids, int64_t replay_row_stride,
+                                        int T, int E, int K, int scoring, int norm_topk_prob, float scaling,
+                                        float* router_weights, float* topk_weights, int64_t* topk_ids,
+                                        int32_t* topk_ids_i32, int64_t* tokens_per_expert, void* dispatch_workspace,
+                                        xtb_stream_t stream) {
+  XTB_CHECK_ARG(tokens_per_expert && (T == 0 || replay_ids), "xtb_router_greedy_replay: null pointer");
+  XTB_CHECK_ARG(T >= 0 && E > 0 && K > 0 && replay_row_stride >= K,
+                "xtb_router_greedy_replay: bad shape T=%d E=%d K=%d replay_row_stride=%lld", T, E, K,
+                (long long)replay_row_stride);
+  if (T == 0) {  // an empty micro-batch: no token arrays to address, only the counts to clear
+    XTB_ENSURE_CTX(tokens_per_expert);
+    XTB_CUDA(cudaMemsetAsync(tokens_per_expert, 0, sizeof(int64_t) * E, as_stream(stream)));
+    return XTB_OK;
+  }
+  XTB_CHECK_ARG(!dispatch_workspace || topk_ids_i32, "xtb_router_greedy_replay: the workspace needs topk_ids_i32");
+  return router_greedy_impl(logits, T, E, K, scoring, norm_topk_prob, scaling, router_weights, topk_weights, topk_ids,
+                            topk_ids_i32, tokens_per_expert, dispatch_workspace, stream, replay_ids, replay_row_stride);
+}
+
 extern "C" int xtb_router_greedy_bwd(const float* router_weights, const float* topk_weights,
                                      const int64_t* topk_ids, const float* grad_topk_weights,
                                      const float* grad_router_weights, const float* grad_logits_direct, int T,
@@ -877,10 +932,11 @@ extern "C" int xtb_router_greedy_bwd(const float* router_weights, const float* t
                       grad_logits, st)
 }
 
-extern "C" int xtb_router_noaux(const float* logits, const float* e_score_correction_bias, int T, int E, int K,
-                                int n_group, int topk_group, int norm_topk_prob, float scaling,
-                                float* router_weights, float* topk_weights, int64_t* topk_ids,
-                                int32_t* topk_ids_i32, float* tokens_per_expert_f32, xtb_stream_t stream) {
+static int router_noaux_impl(const float* logits, const float* e_score_correction_bias, int T, int E, int K,
+                             int n_group, int topk_group, int norm_topk_prob, float scaling, float* router_weights,
+                             float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32,
+                             float* tokens_per_expert_f32, const int64_t* replay_ids, int64_t replay_stride,
+                             xtb_stream_t stream) {
   XTB_CHECK_ARG(logits && e_score_correction_bias && router_weights && topk_weights && topk_ids &&
                     tokens_per_expert_f32,
                 "xtb_router_noaux: null pointer");
@@ -898,11 +954,18 @@ extern "C" int xtb_router_noaux(const float* logits, const float* e_score_correc
   XTB_CUDA(cudaMemsetAsync(tokens_per_expert_f32, 0, sizeof(float) * E, st));
   if (T == 0) return XTB_OK;
   const int blocks = (T + 7) / 8;
-#define XTB_NOAUX(V)                                                                                         \
-  router_noaux_kernel<V><<<blocks, 256, E * sizeof(int), st>>>(logits, e_score_correction_bias, T, E, K, n_group, \
-                                                               topk_group, norm_topk_prob, scaling,             \
-                                                               router_weights, topk_weights, topk_ids,          \
-                                                               topk_ids_i32, tokens_per_expert_f32)
+#define XTB_NOAUX(V)                                                                                                  \
+  if (replay_ids) {                                                                                                   \
+    XTB_CUDA(launch_pdl(router_noaux_kernel<V, true>, dim3(blocks), dim3(256), E * sizeof(int), st, logits,           \
+                        e_score_correction_bias, T, E, K, n_group, topk_group, norm_topk_prob, scaling,               \
+                        router_weights, topk_weights, topk_ids, topk_ids_i32, tokens_per_expert_f32, replay_ids,      \
+                        replay_stride));                                                                              \
+  } else {                                                                                                            \
+    router_noaux_kernel<V><<<blocks, 256, E * sizeof(int), st>>>(logits, e_score_correction_bias, T, E, K, n_group,   \
+                                                                 topk_group, norm_topk_prob, scaling,                 \
+                                                                 router_weights, topk_weights, topk_ids,              \
+                                                                 topk_ids_i32, tokens_per_expert_f32);                \
+  }
   switch (vpl) {
     case 1: XTB_NOAUX(1); break;
     case 2: XTB_NOAUX(2); break;
@@ -914,6 +977,34 @@ extern "C" int xtb_router_noaux(const float* logits, const float* e_score_correc
 #undef XTB_NOAUX
   XTB_LAUNCH_OK();
   return XTB_OK;
+}
+
+extern "C" int xtb_router_noaux(const float* logits, const float* e_score_correction_bias, int T, int E, int K,
+                                int n_group, int topk_group, int norm_topk_prob, float scaling,
+                                float* router_weights, float* topk_weights, int64_t* topk_ids,
+                                int32_t* topk_ids_i32, float* tokens_per_expert_f32, xtb_stream_t stream) {
+  return router_noaux_impl(logits, e_score_correction_bias, T, E, K, n_group, topk_group, norm_topk_prob, scaling,
+                           router_weights, topk_weights, topk_ids, topk_ids_i32, tokens_per_expert_f32, nullptr, 0,
+                           stream);
+}
+
+extern "C" int xtb_router_noaux_replay(const float* logits, const float* e_score_correction_bias,
+                                       const int64_t* replay_ids, int64_t replay_row_stride, int T, int E, int K,
+                                       int n_group, int topk_group, int norm_topk_prob, float scaling,
+                                       float* router_weights, float* topk_weights, int64_t* topk_ids,
+                                       int32_t* topk_ids_i32, float* tokens_per_expert_f32, xtb_stream_t stream) {
+  XTB_CHECK_ARG(tokens_per_expert_f32 && (T == 0 || replay_ids), "xtb_router_noaux_replay: null pointer");
+  XTB_CHECK_ARG(T >= 0 && E > 0 && K > 0 && replay_row_stride >= K,
+                "xtb_router_noaux_replay: bad shape T=%d E=%d K=%d replay_row_stride=%lld", T, E, K,
+                (long long)replay_row_stride);
+  if (T == 0) {  // an empty micro-batch: no token arrays to address, only the counts to clear
+    XTB_ENSURE_CTX(tokens_per_expert_f32);
+    XTB_CUDA(cudaMemsetAsync(tokens_per_expert_f32, 0, sizeof(float) * E, as_stream(stream)));
+    return XTB_OK;
+  }
+  return router_noaux_impl(logits, e_score_correction_bias, T, E, K, n_group, topk_group, norm_topk_prob, scaling,
+                           router_weights, topk_weights, topk_ids, topk_ids_i32, tokens_per_expert_f32, replay_ids,
+                           replay_row_stride, stream);
 }
 
 extern "C" int xtb_router_noaux_bwd(const float* logits, const float* e_score_correction_bias,

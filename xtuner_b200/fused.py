@@ -21,7 +21,7 @@ from torch import Tensor, nn
 
 from . import _capi, ops
 from ._capi import check, current_stream, ptr
-from .router import SCORING
+from .router import SCORING, replay_ids_arg
 
 # Where the next expert-weight gradients are written: a callable returning ``(g_w13_buffer, g_w2_buffer)`` (bf16, same
 # numel as the weights) or None.  The FSDP engine (fsdp_experts.py) points this at its symmetric gradient buffers so the
@@ -39,10 +39,12 @@ def _weight_grad_buffers(w13: Tensor, w2: Tensor):
     return torch.empty_like(w13), torch.empty_like(w2)
 
 
-def _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm, scaling, st):
+def _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm, scaling, st, replay=None):
     """(logits, rw, tw, ids, ids32, tpe, ws): gate, greedy router and dispatch bucketing into the permute workspace ``ws``.
     One launch (xtb_gate_route_dispatch: gate on the tensor cores) where E <= 8, K <= 8, H % 128 == 0 and H <= 4096, the
-    gate and the router as two calls otherwise (their A/B at the shapes both take has not been repeated on H100)."""
+    gate and the router as two calls otherwise (their A/B at the shapes both take has not been repeated on H100).  With
+    ``replay`` (rollout-routed experts, int64 [T, K]) the replay entries of the same two paths gather the weights at those
+    ids instead of a top-k."""
     dev = x.device
     logits = torch.empty((T, E), dtype=torch.float32, device=dev)
     rw = torch.empty((T, E), dtype=torch.float32, device=dev)
@@ -51,7 +53,17 @@ def _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm, scaling, st):
     ids32 = torch.empty((T, K), dtype=torch.int32, device=dev)
     tpe = torch.empty((E,), dtype=torch.int64, device=dev)
     ws = ops.permute_workspace(T, K, E, dev)
-    if E <= 8 and K <= 8 and H % 128 == 0 and H <= 4096:
+    one_launch = E <= 8 and K <= 8 and H % 128 == 0 and H <= 4096
+    if replay is not None:
+        rp, stride = replay_ids_arg(replay, T, K, dev)
+        if one_launch:
+            _k(lib, "xtb_gate_route_replay_dispatch", ptr(x), ptr(gate_w), ptr(rp), stride, T, H, E, K, scoring, int(norm),
+               float(scaling), ptr(logits), ptr(rw), ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
+        else:
+            _k(lib, "xtb_gate_logits", ptr(x), ptr(gate_w), None, ptr(logits), T, H, E, st)
+            _k(lib, "xtb_router_greedy_replay", ptr(logits), ptr(rp), stride, T, E, K, scoring, int(norm), float(scaling),
+               ptr(rw), ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
+    elif one_launch:
         _k(lib, "xtb_gate_route_dispatch", ptr(x), ptr(gate_w), T, H, E, K, scoring, int(norm), float(scaling),
            ptr(logits), ptr(rw), ptr(tw), ptr(ids), ptr(ids32), ptr(tpe), ptr(ws), st)
     else:
@@ -100,7 +112,8 @@ def _k(lib, name: str, *args) -> None:
 class FusedMoEFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x: Tensor, residual: Optional[Tensor], gate_w: Tensor, w13: Tensor, w2: Tensor, top_k: int,
-                norm_topk_prob: bool, scaling: float, hidden_factor: float, scoring: int):
+                norm_topk_prob: bool, scaling: float, hidden_factor: float, scoring: int,
+                rollout_routed_experts: Optional[Tensor] = None):
         lib = _capi.ensure_init()
         st = current_stream()
         T, H = x.shape
@@ -111,7 +124,8 @@ class FusedMoEFunction(torch.autograd.Function):
         dev = x.device
         bf = torch.bfloat16
 
-        logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st)
+        logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st,
+                                                          rollout_routed_experts)
 
         x_perm = torch.empty((M, H), dtype=bf, device=dev)
         row_id_map = torch.empty((M,), dtype=torch.int32, device=dev)
@@ -171,7 +185,7 @@ class FusedMoEFunction(torch.autograd.Function):
         _k(lib, "xtb_moe_combine", ptr(g_xp), ptr(row_id_map), None, ptr(g_x_gate), 1.0, T, K, H, ptr(g_x), st)
 
         g_res = g_out if has_res else None
-        return g_x, g_res, g_gate_w, g_w13, g_w2, None, None, None, None, None
+        return g_x, g_res, g_gate_w, g_w13, g_w2, None, None, None, None, None, None
 
 
 class FusedMoEBlockFunction(torch.autograd.Function):
@@ -181,7 +195,8 @@ class FusedMoEBlockFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, h: Tensor, norm_w: Tensor, eps: float, gate_w: Tensor, w13: Tensor, w2: Tensor, top_k: int,
-                norm_topk_prob: bool, scaling: float, hidden_factor: float, scoring: int):
+                norm_topk_prob: bool, scaling: float, hidden_factor: float, scoring: int,
+                rollout_routed_experts: Optional[Tensor] = None):
         lib = _capi.ensure_init()
         st = current_stream()
         T, H = h.shape
@@ -197,7 +212,8 @@ class FusedMoEBlockFunction(torch.autograd.Function):
         # the norm as its own streaming kernel: folding the gate into it (xtb_rmsnorm_gate with gate_w) is not used by
         # the fused layer (not measured on H100)
         _k(lib, "xtb_rmsnorm_gate", ptr(h), ptr(norm_w), None, float(eps), T, H, E, ptr(x), ptr(rstd), None, st)
-        logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st)
+        logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st,
+                                                          rollout_routed_experts)
         x_perm = torch.empty((M, H), dtype=bf, device=dev)
         row_id_map = torch.empty((M,), dtype=torch.int32, device=dev)
         _k(lib, "xtb_moe_permute_prepared", ptr(x), ptr(ids32), T, K, E, H * 2, ptr(x_perm), ptr(row_id_map), None, ptr(ws), st)
@@ -252,7 +268,7 @@ class FusedMoEBlockFunction(torch.autograd.Function):
         wsn = ops._scratch("norm_bwd", int(lib.xtb_moe_dispatch_bwd_rmsnorm_workspace_bytes(T, H)), dev) if need_nw else None
         _k(lib, "xtb_moe_dispatch_bwd_rmsnorm", ptr(g_xp), ptr(row_id_map), ptr(g_x_gate), ptr(h), ptr(rstd), ptr(norm_w),
            ptr(g_out), T, K, H, ptr(g_h), ptr(g_norm_w), ptr(wsn), st)
-        return g_h, g_norm_w, None, g_gate_w, g_w13, g_w2, None, None, None, None, None
+        return g_h, g_norm_w, None, g_gate_w, g_w13, g_w2, None, None, None, None, None, None
 
 
 _FUSED_NORM_H = (256, 512, 1024, 2048)
@@ -260,9 +276,10 @@ _FUSED_NORM_H = (256, 512, 1024, 2048)
 
 def fused_moe_block(h: Tensor, norm_weight: Tensor, eps: float, gate_weight: Tensor, w13: Tensor, w2: Tensor, *, top_k: int,
                     norm_topk_prob: bool = True, router_scaling_factor: float = 1.0, hidden_factor: float = 1.0,
-                    scoring_func: str = "softmax"):
+                    scoring_func: str = "softmax", rollout_routed_experts: Optional[Tensor] = None):
     """``h`` [T,H] bf16 residual stream -> ``moe(rms_norm(h, norm_weight, eps)) * hidden_factor + h``.
-    Supported H for the fused backward: 256/512/1024/2048.  Returns ``(hidden_states, router_results)``."""
+    Supported H for the fused backward: 256/512/1024/2048.  ``rollout_routed_experts`` (int64 [T, top_k], on h's device):
+    route those experts instead of the router's top-k (RL routing replay).  Returns ``(hidden_states, router_results)``."""
     if not h.is_cuda:
         raise _capi.XtbError("fused_moe_block needs CUDA tensors (no CPU fallback)")
     if h.dtype != torch.bfloat16 or w13.dtype != torch.bfloat16 or w2.dtype != torch.bfloat16:
@@ -272,22 +289,24 @@ def fused_moe_block(h: Tensor, norm_weight: Tensor, eps: float, gate_weight: Ten
         # the fused norm kernels keep the row slice in registers (xtb_rmsnorm_gate: H in 256/512/1024/2048): compose instead
         x = torch.nn.functional.rms_norm(h, (shape[-1],), norm_weight.to(h.dtype), eps)
         return fused_moe(x, h, gate_weight, w13, w2, top_k=top_k, norm_topk_prob=norm_topk_prob,
-                         router_scaling_factor=router_scaling_factor, hidden_factor=hidden_factor, scoring_func=scoring_func)
+                         router_scaling_factor=router_scaling_factor, hidden_factor=hidden_factor, scoring_func=scoring_func,
+                         rollout_routed_experts=rollout_routed_experts)
     h2 = h.contiguous().view(-1, shape[-1])
     gw = gate_weight if gate_weight.dtype == torch.float32 else gate_weight.float()
     nw = norm_weight if norm_weight.dtype == torch.float32 else norm_weight.float()
     out, logits, rw, ids, tpe = FusedMoEBlockFunction.apply(
         h2, nw.contiguous(), eps, gw.contiguous(), w13.contiguous(), w2.contiguous(), top_k, norm_topk_prob,
-        router_scaling_factor, hidden_factor, SCORING[scoring_func])
+        router_scaling_factor, hidden_factor, SCORING[scoring_func], rollout_routed_experts)
     rr = {"logits": logits, "router_weights": rw, "topk_weights": None, "topk_ids": ids, "topkens_per_expert": tpe}
     return out.view(shape), rr
 
 
 def fused_moe(x: Tensor, residual: Optional[Tensor], gate_weight: Tensor, w13: Tensor, w2: Tensor, *, top_k: int,
               norm_topk_prob: bool = True, router_scaling_factor: float = 1.0, hidden_factor: float = 1.0,
-              scoring_func: str = "softmax"):
+              scoring_func: str = "softmax", rollout_routed_experts: Optional[Tensor] = None):
     """``x`` [T,H] bf16 (post-attention-layernorm activations), ``residual`` [T,H] bf16 or None,
-    ``gate_weight`` [E,H] (used in fp32), ``w13`` [E*2I,H] or [E,2I,H], ``w2`` [E*H,I] or [E,H,I] (bf16).
+    ``gate_weight`` [E,H] (used in fp32), ``w13`` [E*2I,H] or [E,2I,H], ``w2`` [E*H,I] or [E,H,I] (bf16),
+    ``rollout_routed_experts`` int64 [T, top_k] or None (RL routing replay, as in :func:`fused_moe_block`).
     Returns ``(hidden_states, router_results)`` with the reference's RouterResults keys."""
     if not x.is_cuda:
         raise _capi.XtbError("fused_moe needs CUDA tensors (no CPU fallback)")
@@ -299,7 +318,7 @@ def fused_moe(x: Tensor, residual: Optional[Tensor], gate_weight: Tensor, w13: T
     gw = gate_weight if gate_weight.dtype == torch.float32 else gate_weight.float()
     out, logits, rw, ids, tpe = FusedMoEFunction.apply(
         x2, res2, gw.contiguous(), w13.contiguous(), w2.contiguous(), top_k, norm_topk_prob, router_scaling_factor,
-        hidden_factor, SCORING[scoring_func])
+        hidden_factor, SCORING[scoring_func], rollout_routed_experts)
     rr = {"logits": logits, "router_weights": rw, "topk_weights": None, "topk_ids": ids, "topkens_per_expert": tpe}
     return out.view(shape), rr
 

@@ -12,8 +12,9 @@
 
 With ``fused=True`` the MoE half of every eligible layer (``post_attention_layernorm`` -> gate -> router -> dispatch ->
 experts -> combine -> ``* hidden_factor + residual``, ``moe_decoder_layer.py:668-705,411-488``) additionally runs as ONE
-autograd node (:func:`xtuner_b200.fused.fused_moe_block`), the form ``bench.py`` measures; the per-op classes above stay
-installed for the paths the fused node does not cover (micro-batched forward, rollout-routed experts).
+autograd node (:func:`xtuner_b200.fused.fused_moe_block`), the form ``bench.py`` measures, rollout-routed experts (RL
+routing replay) included; the per-op classes above stay installed for the path the fused node does not cover
+(micro-batched forward).
 
 Everything else of the model (attention, norms, lm_head, FSDP wrapping, checkpoint keys) is untouched;
 ``install_lm_head_loss()`` separately moves the lm_head cross-entropy onto this package's kernels, and
@@ -104,18 +105,25 @@ def _fused_eligible(layer: nn.Module) -> bool:
 def _fused_layer_forward(self, hidden_states, seq_ctx, position_embeddings):
     """Replacement for ``MoEDecoderLayer._forward`` (``moe_decoder_layer.py:392-488``): the attention half is the
     reference's own modules (``_pre_moe_forward`` lines 634-666), the MoE half one fused autograd node."""
-    if getattr(seq_ctx, "rollout_routed_experts", None) is not None:
-        return type(self)._forward(self, hidden_states, seq_ctx, position_embeddings)  # RL replay routing: per-op path
     residual = hidden_states
     hidden_states = self.input_layernorm(hidden_states)
     attn_outputs = self.self_attn(hidden_states=hidden_states, position_embeddings=position_embeddings, seq_ctx=seq_ctx)
     hidden_states = residual + attn_outputs["projected_output"]
     router = self.gate.router
+    # RL routing replay: this layer's slice of the [S, L, K] ids, moved to the device if offloaded, exactly as the
+    # reference does (moe_decoder_layer.py:669-677)
+    replay = {}  # the keyword only when there are ids: the routing call keeps fused_moe_block's own defaults
+    ids = getattr(seq_ctx, "rollout_routed_experts", None)
+    if ids is not None and self.layer_idx < ids.shape[1]:
+        ids = ids[:, self.layer_idx, :]
+        if seq_ctx.offload_rollout_routed_experts and ids.device != hidden_states.device:
+            ids = ids.contiguous().to(hidden_states.device)
+        replay["rollout_routed_experts"] = ids
     out, rr = _fused.fused_moe_block(
         hidden_states, _local(self.post_attention_layernorm.weight), self.post_attention_layernorm.variance_epsilon,
         _local(self.gate.weight), _local(self.experts.fused_w1w3.weight), _local(self.experts.fused_w2.weight),
         top_k=router.top_k, norm_topk_prob=router.norm_topk_prob, router_scaling_factor=router.router_scaling_factor,
-        hidden_factor=self.hidden_factor, scoring_func=router.scoring_func,
+        hidden_factor=self.hidden_factor, scoring_func=router.scoring_func, **replay,
     )
     return out, rr["logits"], rr["router_weights"], rr["topk_ids"]
 
