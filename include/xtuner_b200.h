@@ -146,10 +146,14 @@ int xtb_router_gate_bwd(const float* router_weights, const float* topk_weights, 
                         void* workspace, xtb_stream_t stream);
 
 /* ---- a2' NoAuxRouter.forward: module/router/noaux_router.py:78-150 (DeepSeek-V3 style) --------------
- * sigmoid scores; choice scores = scores + bias; group-limited routing (top-2 sum per group, keep
- * topk_group groups); topk on masked choice scores; weights gathered from the UNBIASED scores, renormalised
- * with +1e-20 and scaled; router_weights = masked choice scores / row sum; tokens_per_expert as FLOAT32
- * (the reference calls histc on `topk_ids.float()`, :137-142). */
+ * sigmoid scores; choice scores = scores + bias; group-limited routing (group score = top-2 sum of its choice
+ * scores; keep topk_group distinct groups by (score desc, index asc), so when fewer than topk_group groups score
+ * above -inf the lowest-index remaining groups are kept); topk on masked choice scores; weights gathered from the
+ * UNBIASED scores, renormalised with +1e-20 and scaled; router_weights = masked choice scores / row sum;
+ * tokens_per_expert as FLOAT32 (the reference calls histc on `topk_ids.float()`, :137-142).
+ * E a multiple of 32 and <= 512, K <= 32, n_group <= 32 dividing E, group size E / n_group a power of two and a
+ * multiple of E / 32; with a group mask (topk_group < n_group) a group needs at least 2 experts — the reference's
+ * top-2 refuses groups of 1.  XTB_ERR_INVALID otherwise. */
 int xtb_router_noaux(const float* logits, const float* e_score_correction_bias, int T, int E, int K, int n_group,
                      int topk_group, int norm_topk_prob, float scaling, float* router_weights,
                      float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32, float* tokens_per_expert_f32,
@@ -168,8 +172,9 @@ int xtb_router_noaux_replay(const float* logits, const float* e_score_correction
 /* backward of a2' (what autograd does to noaux_router.py:80-134; closed form in oracle/moe_oracle.py
  * noaux_router_bwd).  Inputs are the forward's inputs and outputs, and its group geometry as
  * group_spec = XTB_NOAUX_GROUP_SPEC(n_group, topk_group): 0 when n_group == topk_group (no group mask), otherwise
- * n_group | topk_group << 8.  The kept-group mask is recomputed from logits and bias: a kept expert's router weight may
- * be exactly 0, so router_weights != 0 does not identify it.  Either grad may be NULL. */
+ * n_group | topk_group << 8, with the forward's limits on the group geometry.  The kept-group mask is recomputed from
+ * logits and bias by the forward's own rule: a kept expert's router weight may be exactly 0, so router_weights != 0 does
+ * not identify it.  Either grad may be NULL. */
 #define XTB_NOAUX_GROUP_SPEC(n_group, topk_group) \
   ((n_group) == (topk_group) ? 0 : ((n_group) | ((topk_group) << 8)))
 int xtb_router_noaux_bwd(const float* logits, const float* e_score_correction_bias, const float* router_weights,

@@ -7,12 +7,14 @@ warm-up, with the card name and power limit read in the same run:
              work and their outputs and gradients must be equal bit for bit (checked before timing).
   router     the router alone, forward + backward, at E = 128, K = 8, T = 8192: GreedyRouter routed, GreedyRouter
              replayed, and the reference's eager GreedyRouter replayed (greedy.py:64-98; from oracle/_ref).
+  noaux      NoAuxRouter alone, forward + backward, routed and replayed, at the DeepSeek-V3 geometry (T = 16384,
+             E = 256, K = 8, n_group = 8, topk_group = 4, scaling 2.5).
 
 Prints one line per arm (ms per forward + backward, host dispatch included: median, min and max over the repeats; for
 the router arms also the summed device time of their kernels, from torch.profiler in a run of its own) and a JSON line.  Needs a GPU;
 the reference arm needs oracle/_ref (built by build()).
 
-    python scripts/router_replay_bench.py [--repeats 7 --iters 20 --warmup 5]
+    python scripts/router_replay_bench.py [--repeats 7 --iters 20 --warmup 5] [--only block|router|noaux]
 """
 from __future__ import annotations
 
@@ -134,27 +136,59 @@ def router_arms(T, E, K):
     return arms
 
 
-def main() -> None:
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--repeats", type=int, default=7)
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("router_replay_bench: needs a CUDA device")
-    res = {"card": card(), "arms": {}}
-    for name, shape in (("block_c2", (8192, 2048, 768, 8, 2)), ("block_qwen3_30b_a3b", (8192, 2048, 768, 128, 8))):
-        t = time_arms(block_arms(*shape), a.repeats, a.iters, a.warmup)
-        res["arms"][name] = {"shape": dict(zip("THIEK", shape)), **t}
-        torch.cuda.empty_cache()
-    arms = router_arms(8192, 128, 8)
+def noaux_arms(T, E, K, n_group, topk_group):
+    from xtuner_b200 import router
+
+    g = torch.Generator(device=DEV).manual_seed(2)
+    logits = torch.randn(T, E, generator=g, device=DEV).requires_grad_(True)
+    ids = torch.randint(0, E, (T, 3, K), generator=g, device=DEV)[:, 1, :]  # the layer slice of an [S, L, K] tensor
+    g_tw = torch.randn(T, K, generator=g, device=DEV)
+    g_rw = torch.randn(T, E, generator=g, device=DEV)
+    r = router.NoAuxRouter(n_routed_experts=E, num_experts_per_tok=K, router_scaling_factor=2.5,
+                           scoring_func="sigmoid", n_group=n_group, topk_group=topk_group).to(DEV)
+    r.e_score_correction_bias.copy_(torch.randn(E, generator=g, device=DEV) * 0.1)
+
+    def arm(replay):
+        def step():
+            logits.grad = None
+            res = r(logits, replay)
+            torch.autograd.backward((res["topk_weights"], res["router_weights"]), (g_tw, g_rw))
+        return step
+
+    return {"noaux_routed": arm(None), "noaux_replayed": arm(ids)}
+
+
+def router_only(arms: dict, a) -> dict:
     t = time_arms(arms, a.repeats, a.iters * 5, a.warmup)
     # the router alone is a few microseconds of device work: host dispatch sets the wall time, so the kernels' own
     # device time is reported beside it
     ku = kernel_us(arms, a.iters)
     for k in t:
         t[k]["kernel_us"] = ku[k]
-    res["arms"]["router_e128_k8"] = {"shape": {"T": 8192, "E": 128, "K": 8}, **t}
+    return t
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--repeats", type=int, default=7)
+    ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--only", choices=("block", "router", "noaux"), default=None, help="one group of arms")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("router_replay_bench: needs a CUDA device")
+    res = {"card": card(), "arms": {}}
+    if a.only in (None, "block"):
+        for name, shape in (("block_c2", (8192, 2048, 768, 8, 2)), ("block_qwen3_30b_a3b", (8192, 2048, 768, 128, 8))):
+            t = time_arms(block_arms(*shape), a.repeats, a.iters, a.warmup)
+            res["arms"][name] = {"shape": dict(zip("THIEK", shape)), **t}
+            torch.cuda.empty_cache()
+    if a.only in (None, "router"):
+        res["arms"]["router_e128_k8"] = {"shape": {"T": 8192, "E": 128, "K": 8},
+                                         **router_only(router_arms(8192, 128, 8), a)}
+    if a.only in (None, "noaux"):
+        shape = {"T": 16384, "E": 256, "K": 8, "n_group": 8, "topk_group": 4}
+        res["arms"]["noaux_deepseek_v3"] = {"shape": shape, **router_only(noaux_arms(*shape.values()), a)}
     for group, d in res["arms"].items():
         for arm, v in d.items():
             if isinstance(v, dict) and "ms_median" in v:

@@ -17,7 +17,8 @@ of tests/router_reference.py, at the edges the parity tests of tests/test_gpu_ro
   with every null combination of the three gradients; the
   gate backward (both small kernels, the strided pair, colsum) against float64 on both sides of 768 tokens per block.
 * No-aux router: E = 32 to 512, K up to 32, lanes per group 1 to 8, no mask, tied group scores, negative-bias kept
-  experts against masked zeros, the zero-score kept expert's gradient, NaN rows, refusals.
+  experts against masked zeros, the zero-score kept expert's gradient, whole groups with a -inf bias (fewer than
+  topk_group groups above -inf: exactly topk_group are still kept, routed and replayed), NaN rows, refusals.
 * Determinism and T = 0.
 
 Outputs go to views with 16 NaN-filled guard rows on each side; the guards must stay as they were."""
@@ -536,6 +537,46 @@ def test_noaux_zero_score_kept_expert_gradient():
     torch.testing.assert_close(got.double(), ref, rtol=1e-4, atol=1e-6)
 
 
+def noaux_replay(lg, bias, ids, NG, TG, norm=True, scaling=2.5):
+    T, E = lg.shape
+    K = ids.shape[1]
+    rw, tw = Guarded(T, E), Guarded(T, K)
+    oids, i32 = Guarded(T, K, torch.int64), Guarded(T, K, torch.int32)
+    tpe = torch.full((E,), -1.0, device="cuda")
+    _ok(_lib().xtb_router_noaux_replay(_p(lg), _p(bias), _p(ids), ids.stride(0), T, E, K, NG, TG, int(norm), scaling,
+                                       _p(rw.v), _p(tw.v), _p(oids.v), _p(i32.v), _p(tpe), _st()),
+        "xtb_router_noaux_replay")
+    return dict(rw=rw.check("noaux replay rw"), tw=tw.check("noaux replay tw"))
+
+
+@pytest.mark.parametrize("E,NG,TG,K,finite", [(256, 8, 4, 8, (0, 1)), (256, 8, 4, 8, (6,)), (64, 8, 3, 12, (5,)),
+                                              (512, 16, 4, 8, ()), (32, 16, 3, 2, (3, 9))])
+def test_noaux_groups_scoring_minus_inf(E, NG, TG, K, finite):
+    """Every group but ``finite`` has a -inf bias, so fewer than topk_group groups score above -inf.  The forward still
+    keeps exactly topk_group groups: those above -inf, then the lowest-index others (oracle.noaux_kept_experts), as the
+    backward does.  A kept -inf group makes the row sum -inf, so router_weights are NaN at its experts and 0 elsewhere;
+    replaying the forward's ids gives the same router_weights and topk weights."""
+    T = 64
+    g = torch.Generator(device="cuda").manual_seed(E + TG + len(finite))
+    # distinct logits 6 / E apart in every row: the top-k is decided in fp32 as in float64
+    lg = (torch.rand(T, E, generator=g, device="cuda").argsort(-1).float() - E / 2) * (6 / E)
+    bias = torch.full((NG, E // NG), -torch.inf, device="cuda")
+    bias[list(finite)] = 0.0
+    bias = bias.view(E)
+    r = noaux(lg, bias, K, NG, TG)
+    ids64, kept, masked = R.noaux_ref(lg, bias, K, NG, TG)
+    others = [i for i in range(NG) if i not in finite]
+    want_groups = torch.zeros(NG, dtype=torch.bool)
+    want_groups[list(finite) + others[: TG - len(finite)]] = True
+    assert bool((kept.view(T, NG, -1).all(-1).cpu() == want_groups).all())
+    assert torch.equal(r["ids"], ids64)
+    assert torch.equal(r["tpe"], torch.bincount(r["ids"].reshape(-1), minlength=E).float())
+    torch.testing.assert_close(r["rw"].double(), masked / masked.sum(-1, keepdim=True), rtol=0, atol=0, equal_nan=True)
+    rp = noaux_replay(lg, bias, r["ids"], NG, TG)
+    assert torch.equal(rp["rw"].view(torch.int32), r["rw"].view(torch.int32))
+    assert torch.equal(rp["tw"].view(torch.int32), r["tw"].view(torch.int32))
+
+
 def test_noaux_nan_rows_and_refusals():
     from xtuner_b200._capi import XtbError
 
@@ -551,7 +592,8 @@ def test_noaux_nan_rows_and_refusals():
         srt = ids.sort(-1).values
         assert bool((srt[:, 1:] != srt[:, :-1]).all())
         assert int(r["tpe"].sum()) == 16 * K
-    for E2, K2, NG, TG in [(96, 4, 1, 1), (192, 4, 3, 1), (64, 33, 1, 1)]:
+    # (32, 32, 4): a group mask over groups of one expert, whose second-best score would be -inf in every group
+    for E2, K2, NG, TG in [(96, 4, 1, 1), (192, 4, 3, 1), (64, 33, 1, 1), (32, 2, 32, 4)]:
         with pytest.raises(XtbError):
             noaux(torch.zeros(4, E2, device="cuda"), torch.zeros(E2, device="cuda"), K2, NG, TG)
     # the backward refuses a group_spec that is not the forward's geometry (1 was the old "has a group mask" flag)
@@ -560,6 +602,10 @@ def test_noaux_nan_rows_and_refusals():
     for spec in (1, 3 | 2 << 8, 8 | 8 << 8, 8 | 0 << 8):
         with pytest.raises(XtbError):
             noaux_bwd(lg, bias, r, K, 8, 4, None, g_rw, group_spec=spec)
+    lg32, b32 = torch.randn(16, 32, device="cuda"), torch.zeros(32, device="cuda")
+    r32 = noaux(lg32, b32, 2, 32, 32)  # groups of one expert without a mask are accepted
+    with pytest.raises(XtbError):
+        noaux_bwd(lg32, b32, r32, 2, 32, 4, None, torch.randn(16, 32, device="cuda"), group_spec=32 | 4 << 8)
 
 
 # ---- general ---------------------------------------------------------------------------------------------------------

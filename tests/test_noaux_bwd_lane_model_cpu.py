@@ -2,8 +2,10 @@
 consecutive experts, xor-shuffle reductions for the row sums, the group mask recomputed from the choice scores
 (``noaux_kept_experts``: per-lane top-2, xor merges across the lanes of a group, topk_group butterfly arg-max rounds),
 the top-k gradient scattered by id.  Restates the kernel's per-lane arithmetic and checks it against the reference-made
-gradient fixture and against the forward's group choice — the kernel itself is covered on the GPU by
-tests/test_gpu_router.py and tests/test_gpu_router_edges.py."""
+gradient fixture.  ``noaux_kept_experts`` is also the forward's group mask (``router_noaux_kernel`` calls it with
+LPT = 32, VPL = E / 32), so its model is checked against the oracle's group choice under both lane mappings, on rows
+where whole groups score -inf too.  The kernels themselves are covered on the GPU by tests/test_gpu_router.py and
+tests/test_gpu_router_edges.py."""
 import numpy as np
 import pytest
 import torch
@@ -20,11 +22,43 @@ def top2_insert(a, b, v):
 
 
 def kept_lane_model(ch, n_group, topk_group, LPT, VPL):
-    """``noaux_kept_experts<LPT, VPL>`` for one token: ``ch`` float32 [E] -> bool [E]."""
+    """``noaux_kept_experts<LPT, VPL>`` for one token: ``ch`` float32 [E] -> bool [E].  The backward's group mask at
+    ``dispatch(E)``, the forward's at ``(32, E // 32)``.  With LPT = 32 (the forward, and the backward at E = 256 and
+    512) the kernel takes its one-candidate-per-lane path; otherwise the slot loop."""
     E = ch.shape[0]
     f32 = np.float32
     gs = E // n_group
     ninf = f32(-np.inf)
+    if LPT == 32:  # one candidate per lane: the lane's group g, scored on the group's first lane
+        assert VPL == E // 32 and gs % VPL == 0
+        a = np.full(LPT, ninf, f32)
+        b = np.full(LPT, ninf, f32)
+        for sub in range(LPT):
+            for j in range(VPL):
+                a[sub], b[sub] = top2_insert(a[sub], b[sub], ch[sub * VPL + j])
+        o = 1
+        while o < gs // VPL:
+            oa, ob = a[np.arange(LPT) ^ o], b[np.arange(LPT) ^ o]
+            a, b = np.maximum(a, oa), np.maximum(np.minimum(a, oa), np.maximum(b, ob))
+            o *= 2
+        gv = (a + b).astype(f32)
+        grp = np.arange(LPT) * VPL // gs
+        cand = np.arange(LPT) * VPL % gs == 0
+        kept = set()
+        for _ in range(topk_group):
+            ok = cand & ~np.isin(grp, list(kept)) & (gv >= ninf)
+            bv = np.where(ok, gv, ninf).astype(f32)
+            bi = np.where(ok, grp, 2**31 - 1).astype(np.int64)
+            o = 16
+            while o > 0:
+                ov, oi = bv[np.arange(LPT) ^ o], bi[np.arange(LPT) ^ o]
+                take = (ov > bv) | ((ov == bv) & (oi < bi))
+                bv, bi = np.where(take, ov, bv), np.where(take, oi, bi)
+                o //= 2
+            assert (bi == bi[0]).all()
+            if bi[0] < n_group:
+                kept.add(int(bi[0]))
+        return np.array([(e // gs) in kept for e in range(E)])
     gv = np.full((LPT, VPL), ninf, f32)
     cand = np.zeros((LPT, VPL), bool)
     a = np.full(LPT, ninf, f32)
@@ -159,12 +193,13 @@ def test_noaux_bwd_lane_model(tag):
 @pytest.mark.parametrize("E,n_group,topk_group", [(32, 4, 2), (32, 16, 3), (64, 8, 3), (128, 32, 5), (256, 8, 4),
                                                   (256, 2, 1), (512, 16, 4), (512, 4, 3), (512, 32, 7)])
 def test_kept_experts_lane_model_equals_the_forward_choice(E, n_group, topk_group):
-    """The backward's recomputed group mask, under the backward's lane mapping (groups inside one lane and groups
-    spanning 2 to 32 lanes), equals the group choice of the forward: the oracle's mask, and the experts the forward's
-    router_weights leave non-zero.  Rows include tied group scores (lowest group index first)."""
+    """The recomputed group mask, under the backward's lane mapping (groups inside one lane and groups spanning 2 to 32
+    lanes) and under the forward's (one warp per token), equals the group choice of the forward: the oracle's mask,
+    and the experts the forward's router_weights leave non-zero.  Rows include tied group scores (lowest group index
+    first) and whole groups scoring -inf, down to every group: exactly topk_group groups are kept all the same, the
+    groups above -inf first, then the lowest-index remaining ones."""
     from oracle import moe_oracle as O
 
-    LPT, VPL = dispatch(E)
     g = torch.Generator().manual_seed(E + n_group)
     T = 6
     logits = torch.randn(T, E, generator=g)
@@ -173,14 +208,27 @@ def test_kept_experts_lane_model_equals_the_forward_choice(E, n_group, topk_grou
     bias = torch.randn(E, generator=g) * 0.1
     ch = torch.sigmoid(logits) + bias
     ch[0] = 0.25
+    gs = E // n_group
+    ninf = ch[2:6].clone().view(4, n_group, gs)
+    ninf[0, :-1] = -torch.inf  # only the last group above -inf
+    ninf[1] = -torch.inf  # every group -inf
+    ninf[2, 1::2] = -torch.inf  # every odd group -inf
+    ninf[3, :, 1:] = -torch.inf  # one score per group above -inf: every group score is -inf
+    ch = torch.cat([ch, ninf.view(4, E)])
     want = O.noaux_kept_experts(ch, n_group, topk_group)
-    for t in range(T):
-        got = kept_lane_model(ch[t].numpy(), n_group, topk_group, LPT, VPL)
-        assert (got == want[t].numpy()).all(), t
-    assert (want.view(T, n_group, -1).all(-1).sum(-1) == topk_group).all()
-    assert torch.equal(want[0].view(n_group, -1).all(-1).nonzero().flatten(), torch.arange(topk_group))
+    for LPT, VPL in (dispatch(E), (32, E // 32)):
+        for t in range(ch.shape[0]):
+            got = kept_lane_model(ch[t].numpy(), n_group, topk_group, LPT, VPL)
+            assert (got == want[t].numpy()).all(), (LPT, VPL, t)
+    kept_groups = want.view(-1, n_group, gs).all(-1)
+    assert (kept_groups.sum(-1) == topk_group).all()
+    assert torch.equal(kept_groups[0].nonzero().flatten(), torch.arange(topk_group))
+    first = torch.arange(topk_group)
+    assert torch.equal(kept_groups[6].nonzero().flatten(), torch.cat([first[:-1], torch.tensor([n_group - 1])]))
+    assert torch.equal(kept_groups[7].nonzero().flatten(), first)
+    assert torch.equal(kept_groups[9].nonzero().flatten(), first)
     fwd = O.noaux_router(logits[2:], bias, min(8, E // n_group * topk_group), n_group, topk_group, 1.0)
-    assert torch.equal(fwd["router_weights"] != 0, want[2:])
+    assert torch.equal(fwd["router_weights"] != 0, want[2:6])
 
 
 def test_zero_score_kept_expert_keeps_its_router_weight_gradient():

@@ -391,171 +391,58 @@ __global__ void __launch_bounds__(256) router_greedy_bwd_kernel(
 }
 
 // =====================================================================================================
-// a2' no-aux router: one warp per token, lane holds VPL = E/32 consecutive experts.
+// a2' no-aux router: the forward is one warp per token, lane holds VPL = E/32 consecutive experts; the backward
+// takes the XTB_ROUTER_DISPATCH lane mapping.
 // =====================================================================================================
-// REPLAY (noaux_router.py:114-121): router_weights as above — they do not depend on the ids — and the topk weights
-// gathered from the unbiased scores at the rows of replay_ids (row stride replay_stride elements) in place of the
-// top-k, which the reference computes and discards.  An id outside [0, E) becomes expert 0 and makes every topk weight
-// of its token NaN.
-template <int VPL, bool REPLAY = false>
-__global__ void __launch_bounds__(256) router_noaux_kernel(const float* __restrict__ logits,
-                                                           const float* __restrict__ bias, int T, int E, int K,
-                                                           int n_group, int topk_group, int norm_topk,
-                                                           float scaling, float* __restrict__ router_weights,
-                                                           float* __restrict__ topk_weights,
-                                                           int64_t* __restrict__ topk_ids,
-                                                           int32_t* __restrict__ topk_ids_i32,
-                                                           float* __restrict__ tokens_per_expert,
-                                                           const int64_t* __restrict__ replay_ids = nullptr,
-                                                           int64_t replay_stride = 0) {
-  if constexpr (REPLAY) pdl_sync();
-  extern __shared__ int s_hist[];
-  for (int i = threadIdx.x; i < E; i += blockDim.x) s_hist[i] = 0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31;
-  const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const bool active = token < T;
-  const int tok = active ? token : T - 1;
-  const int e0 = lane * VPL;
-  const int group_size = E / n_group;
-  const int lanes_per_group = group_size / VPL;  // >= 1 (checked on the host)
-  const int my_group = lane / lanes_per_group;
-
-  float sc[VPL], ch[VPL];
-#pragma unroll
-  for (int j = 0; j < VPL; ++j) {
-    const float x = logits[(size_t)tok * E + e0 + j];
-    sc[j] = 1.f / (1.f + expf(-x));
-    ch[j] = sc[j] + bias[e0 + j];
-  }
-  if (n_group != topk_group) {
-    // top-2 of the group's choice scores
+// Which of a token's experts the no-aux router's group mask keeps, computed from the choice scores ch = s + b; the
+// forward and the backward both call it.  A group's score is its exact largest plus its exact second largest choice
+// score, and topk_group rounds of (score desc, group index asc) over the groups not kept yet pick topk_group distinct
+// groups; both are independent of how the experts are spread over lanes, so every lane mapping keeps the same groups.
+// A group whose score is -inf (fewer than two of its scores above -inf) is still picked, lowest index first, once no
+// group above -inf is left; only a NaN group score (+inf and -inf in one group: an infinite bias) is never picked.
+// LPT lanes hold VPL consecutive experts each; groups of gs = E / n_group experts (a power of two) either lie whole
+// inside one lane (gs <= VPL) or span gs / VPL neighbouring lanes.  The router weight of a kept expert may be exactly 0
+// (s + b == 0), so router_weights cannot tell kept from masked experts.
+template <int LPT, int VPL>
+__device__ __forceinline__ void noaux_kept_experts(const float (&ch)[VPL], int e0, int E, int n_group, int topk_group,
+                                                   bool (&keep)[VPL]) {
+  const int gs = E / n_group;
+  if constexpr (LPT == 32) {
+    // One warp per token: VPL = E / 32 (the only 32-lane geometry the host accepts with a group mask) divides gs, so
+    // the lane lies inside one group g, whose first lane holds its score: one candidate per lane, and the same rounds
+    // as the slot loop below.
     float a = -INFINITY, b = -INFINITY;  // a >= b
 #pragma unroll
     for (int j = 0; j < VPL; ++j) {
       const float v = ch[j];
       if (v > a) { b = a; a = v; } else if (v > b) { b = v; }
     }
-    for (int o = 1; o < lanes_per_group; o <<= 1) {
+    for (int o = 1; o < gs / VPL; o <<= 1) {
       const float oa = __shfl_xor_sync(0xffffffffu, a, o);
       const float ob = __shfl_xor_sync(0xffffffffu, b, o);
-      // merge two sorted pairs
       const float na = fmaxf(a, oa);
       const float nb = fmaxf(fminf(a, oa), fmaxf(b, ob));
       a = na;
       b = nb;
     }
-    const float gscore = a + b;
-    // lane g (< n_group) takes group g's score
-    float gs = __shfl_sync(0xffffffffu, gscore, min(lane, n_group - 1) * lanes_per_group);
-    if (lane >= n_group) gs = -INFINITY;
-    unsigned sel_groups = 0;
-    bool mine_taken = false;
+    const float gv = a + b;
+    const int g = e0 / gs;
+    const bool cand = (e0 % gs) == 0;
+    unsigned kept = 0;
     for (int r = 0; r < topk_group; ++r) {
-      float bv = mine_taken ? -INFINITY : gs;
-      int bi = lane;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+      float bv = -INFINITY;
+      int bi = 0x7fffffff;
+      if (cand && !((kept >> g) & 1u) && gv >= bv) {  // not NaN: the slot loop's test against the initial (-inf, max)
+        bv = gv;
+        bi = g;
       }
-      sel_groups |= 1u << bi;
-      if (bi == lane) mine_taken = true;
+      group_argmax<32>(bv, bi);
+      if (bi < n_group) kept |= 1u << bi;
     }
-    if (!((sel_groups >> my_group) & 1u)) {
 #pragma unroll
-      for (int j = 0; j < VPL; ++j) ch[j] = 0.0f;  // masked_fill(~mask, 0.0)
-    }
+    for (int j = 0; j < VPL; ++j) keep[j] = (kept >> g) & 1u;
+    return;
   }
-  // router_weights = choice / row-sum
-  float rs = 0.f;
-#pragma unroll
-  for (int j = 0; j < VPL; ++j) rs += ch[j];
-  rs = warp_sum(rs);
-  if (active) {
-#pragma unroll
-    for (int j = 0; j < VPL; ++j) router_weights[(size_t)token * E + e0 + j] = ch[j] / rs;
-  }
-  // top-k over the (masked) choice scores, weights from the unbiased scores
-  float sel_w[32];
-  int sel_e[32];
-  float sum = 0.f;
-  bool bad = false;
-  if constexpr (REPLAY) {
-    const int64_t* ids = replay_ids + tok * replay_stride;
-    for (int k = 0; k < K; ++k) {
-      const int64_t raw = ids[k];
-      const bool ok = raw >= 0 && raw < E;
-      const int id = ok ? (int)raw : 0;
-      float bw = 0.f;
-#pragma unroll
-      for (int j = 0; j < VPL; ++j)
-        if (e0 + j == id) bw = sc[j];
-      bw = warp_sum(bw);  // one lane holds expert id; the others add 0
-      bad |= !ok;
-      sel_w[k] = bw;
-      sel_e[k] = id;
-      sum += bw;
-    }
-  } else {
-    unsigned taken = 0;
-    for (int k = 0; k < K; ++k) {
-      float bv = -INFINITY, bw = 0.f;
-      int be = 0x7fffffff;
-#pragma unroll
-      for (int j = 0; j < VPL; ++j) {
-        if (!((taken >> j) & 1u) && ch[j] > bv) { bv = ch[j]; be = e0 + j; bw = sc[j]; }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-        const int oe = __shfl_xor_sync(0xffffffffu, be, o);
-        const float ow = __shfl_xor_sync(0xffffffffu, bw, o);
-        if (ov > bv || (ov == bv && oe < be)) { bv = ov; be = oe; bw = ow; }
-      }
-      if (be < 0 || be >= E) {  // no score left that compares (NaN or -inf): the lowest index not selected yet, with
-                                // weight 0.  sel_e is the same on every lane, and that index is at most k < K <= E.
-        unsigned used = 0;
-        for (int i = 0; i < k; ++i)
-          if (sel_e[i] < 32) used |= 1u << sel_e[i];
-        be = __ffs(~used) - 1;
-        bw = 0.f;
-      }
-      if (be >= e0 && be < e0 + VPL) taken |= 1u << (be - e0);
-      if (k < 32) { sel_w[k] = bw; sel_e[k] = be; }
-      sum += bw;
-    }
-  }
-  if (active && lane == 0) {
-    const float denom = sum + 1e-20f;
-    for (int k = 0; k < K; ++k) {
-      float wv = sel_w[k];
-      if (K > 1 && norm_topk) wv = wv / denom;
-      wv = wv * scaling;
-      if (REPLAY && bad) wv = __int_as_float(0x7fffffff);  // NaN
-      topk_weights[(size_t)token * K + k] = wv;
-      topk_ids[(size_t)token * K + k] = (int64_t)sel_e[k];
-      if (topk_ids_i32) topk_ids_i32[(size_t)token * K + k] = sel_e[k];
-      atomicAdd(&s_hist[sel_e[k]], 1);
-    }
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < E; i += blockDim.x)
-    if (s_hist[i]) atomicAdd(&tokens_per_expert[i], (float)s_hist[i]);  // exact: integer counts < 2^24
-}
-
-// Which of a token's experts the no-aux router's group mask keeps, recomputed from the choice scores ch = s + b.  A
-// group's score is its exact largest plus its exact second largest choice score, and topk_group rounds of
-// (score desc, group index asc) pick the kept groups; both are independent of how the experts are spread over lanes,
-// so this gives router_noaux_kernel's choice under any lane mapping.  LPT lanes hold VPL consecutive experts each;
-// groups of gs = E / n_group experts (a power of two) either lie whole inside one lane (gs <= VPL) or span gs / VPL
-// neighbouring lanes.  The router weight of a kept expert may be exactly 0 (s + b == 0), so router_weights cannot
-// tell kept from masked experts.
-template <int LPT, int VPL>
-__device__ __forceinline__ void noaux_kept_experts(const float (&ch)[VPL], int e0, int E, int n_group, int topk_group,
-                                                   bool (&keep)[VPL]) {
-  const int gs = E / n_group;
   // gv[j]: score of the group whose last local expert is j (candidate slots); others -inf and not candidates
   float gv[VPL];
   bool cand[VPL];
@@ -571,12 +458,12 @@ __device__ __forceinline__ void noaux_kept_experts(const float (&ch)[VPL], int e
   }
   if (gs > VPL) {  // merge the top-2 pairs of the gs / VPL lanes of the group; its first lane holds the candidate
     for (int o = 1; o < gs / VPL; o <<= 1) {
-      const float oa = __shfl_xor_sync(0xffffffffu, a, o);
-      const float ob = __shfl_xor_sync(0xffffffffu, b, o);
-      const float na = fmaxf(a, oa);
-      const float nb = fmaxf(fminf(a, oa), fmaxf(b, ob));
-      a = na;
-      b = nb;
+        const float oa = __shfl_xor_sync(0xffffffffu, a, o);
+        const float ob = __shfl_xor_sync(0xffffffffu, b, o);
+        const float na = fmaxf(a, oa);
+        const float nb = fmaxf(fminf(a, oa), fmaxf(b, ob));
+        a = na;
+        b = nb;
     }
     gv[VPL - 1] = a + b;
     cand[VPL - 1] = (e0 % gs) == 0;
@@ -593,16 +480,123 @@ __device__ __forceinline__ void noaux_kept_experts(const float (&ch)[VPL], int e
         bi = gi;
       }
     }
-#pragma unroll
-    for (int o = LPT / 2; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-    }
+    group_argmax<LPT>(bv, bi);
     if (bi < n_group) kept |= 1u << bi;
   }
 #pragma unroll
   for (int j = 0; j < VPL; ++j) keep[j] = (kept >> ((e0 + j) / gs)) & 1u;
+}
+
+// Forward.  The group mask is noaux_kept_experts<32, VPL>.  REPLAY (noaux_router.py:114-121): router_weights as
+// routing — they do not depend on the ids — and the topk weights gathered from the unbiased scores at the rows of
+// replay_ids (row stride replay_stride elements) in place of the top-k, which the reference computes and discards.  An
+// id outside [0, E) becomes expert 0 and makes every topk weight of its token NaN.
+template <int VPL, bool REPLAY = false>
+__global__ void __launch_bounds__(256) router_noaux_kernel(const float* __restrict__ logits,
+                                                           const float* __restrict__ bias, int T, int E, int K,
+                                                           int n_group, int topk_group, int norm_topk,
+                                                           float scaling, float* __restrict__ router_weights,
+                                                           float* __restrict__ topk_weights,
+                                                           int64_t* __restrict__ topk_ids,
+                                                           int32_t* __restrict__ topk_ids_i32,
+                                                           float* __restrict__ tokens_per_expert,
+                                                           const int64_t* __restrict__ replay_ids,
+                                                           int64_t replay_stride) {
+  pdl_sync();
+  extern __shared__ int s_hist[];
+  for (int i = threadIdx.x; i < E; i += blockDim.x) s_hist[i] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const bool active = token < T;
+  const int tok = active ? token : T - 1;
+  const int e0 = lane * VPL;
+
+  float sc[VPL], ch[VPL];
+#pragma unroll
+  for (int j = 0; j < VPL; ++j) {
+    const float x = logits[(size_t)tok * E + e0 + j];
+    sc[j] = 1.f / (1.f + expf(-x));
+    ch[j] = sc[j] + bias[e0 + j];
+  }
+  if (n_group != topk_group) {
+    bool keep[VPL];
+    noaux_kept_experts<32, VPL>(ch, e0, E, n_group, topk_group, keep);
+#pragma unroll
+    for (int j = 0; j < VPL; ++j)
+      if (!keep[j]) ch[j] = 0.0f;  // masked_fill(~mask, 0.0)
+  }
+  // router_weights = choice / row-sum
+  float rs = 0.f;
+#pragma unroll
+  for (int j = 0; j < VPL; ++j) rs += ch[j];
+  rs = warp_sum(rs);
+  if (active) {
+#pragma unroll
+    for (int j = 0; j < VPL; ++j) router_weights[(size_t)token * E + e0 + j] = ch[j] / rs;
+  }
+  // top-k over the (masked) choice scores, weights from the unbiased scores.  K <= 32: lane k keeps pick k.
+  float my_w = 0.f;
+  int my_e = 0;
+  float sum = 0.f;
+  bool bad = false;
+  if constexpr (REPLAY) {
+    const int64_t* ids = replay_ids + tok * replay_stride;
+    for (int k = 0; k < K; ++k) {
+      const int64_t raw = ids[k];
+      const bool ok = raw >= 0 && raw < E;
+      const int id = ok ? (int)raw : 0;
+      float bw = 0.f;
+#pragma unroll
+      for (int j = 0; j < VPL; ++j)
+        if (e0 + j == id) bw = sc[j];
+      bw = warp_sum(bw);  // one lane holds expert id; the others add 0
+      bad |= !ok;
+      if (lane == k) { my_w = bw; my_e = id; }
+      sum += bw;
+    }
+  } else {
+    unsigned taken = 0;  // bit j set: expert e0 + j already selected
+    unsigned used = 0;   // bit e set: expert e < 32 already selected (the same on every lane)
+    for (int k = 0; k < K; ++k) {
+      float bv = -INFINITY, bw = 0.f;
+      int be = 0x7fffffff;
+#pragma unroll
+      for (int j = 0; j < VPL; ++j) {
+        if (!((taken >> j) & 1u) && ch[j] > bv) { bv = ch[j]; be = e0 + j; bw = sc[j]; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oe = __shfl_xor_sync(0xffffffffu, be, o);
+        const float ow = __shfl_xor_sync(0xffffffffu, bw, o);
+        if (ov > bv || (ov == bv && oe < be)) { bv = ov; be = oe; bw = ow; }
+      }
+      if (be < 0 || be >= E) {  // no score left that compares (NaN or -inf): the lowest index not selected yet, with
+                                // weight 0; that index is at most k < K <= 32, so `used` tracks it.
+        be = __ffs(~used) - 1;
+        bw = 0.f;
+      }
+      if (be >= e0 && be < e0 + VPL) taken |= 1u << (be - e0);
+      if (be < 32) used |= 1u << be;
+      if (lane == k) { my_w = bw; my_e = be; }
+      sum += bw;
+    }
+  }
+  if (active && lane < K) {
+    const float denom = sum + 1e-20f;
+    float wv = my_w;
+    if (K > 1 && norm_topk) wv = wv / denom;
+    wv = wv * scaling;
+    if (REPLAY && bad) wv = __int_as_float(0x7fffffff);  // NaN
+    topk_weights[(size_t)token * K + lane] = wv;
+    topk_ids[(size_t)token * K + lane] = (int64_t)my_e;
+    if (topk_ids_i32) topk_ids_i32[(size_t)token * K + lane] = my_e;
+    atomicAdd(&s_hist[my_e], 1);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < E; i += blockDim.x)
+    if (s_hist[i]) atomicAdd(&tokens_per_expert[i], (float)s_hist[i]);  // exact: integer counts < 2^24
 }
 
 // backward of the no-aux router (closed form: oracle/moe_oracle.py noaux_router_bwd).  LPT lanes per token, each
@@ -613,6 +607,7 @@ __global__ void __launch_bounds__(256) router_noaux_bwd_kernel(
     const float* __restrict__ topk_weights, const int64_t* __restrict__ topk_ids, const float* __restrict__ g_tw,
     const float* __restrict__ g_rw, int T, int E, int K, int n_group, int topk_group, int norm_topk, float scaling,
     float* __restrict__ grad_logits) {
+  pdl_sync();
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x;
   const int token = gtid / LPT;
   const int sub = threadIdx.x % LPT;
@@ -857,8 +852,8 @@ static int launch_router_noaux_bwd(const float* logits, const float* bias, const
                                    int n_group, int topk_group, int norm, float scaling, float* gl, cudaStream_t st) {
   const int tokens_per_block = 256 / LPT;
   const int blocks = (T + tokens_per_block - 1) / tokens_per_block;
-  router_noaux_bwd_kernel<LPT, VPL><<<blocks, 256, 0, st>>>(logits, bias, rw, tw, ids, g_tw, g_rw, T, E, K, n_group,
-                                                           topk_group, norm, scaling, gl);
+  XTB_CUDA(launch_pdl(router_noaux_bwd_kernel<LPT, VPL>, dim3(blocks), dim3(256), 0, st, logits, bias, rw, tw, ids,
+                      g_tw, g_rw, T, E, K, n_group, topk_group, norm, scaling, gl));
   XTB_LAUNCH_OK();
   return XTB_OK;
 }
@@ -932,6 +927,22 @@ extern "C" int xtb_router_greedy_bwd(const float* router_weights, const float* t
                       grad_logits, st)
 }
 
+// The no-aux router's group geometry, for the forward and the backward alike.  The forward holds E / 32 experts per
+// lane, so a group lies whole inside one lane or spans a power-of-two number of lanes; a group mask scores each group
+// by its top two experts, so its groups need at least two.
+static int check_noaux_groups(const char* who, int E, int n_group, int topk_group) {
+  XTB_CHECK_ARG(E % 32 == 0 && E <= 512, "%s: E=%d must be a multiple of 32 and <= 512", who, E);
+  XTB_CHECK_ARG(n_group >= 1 && n_group <= 32 && E % n_group == 0 && topk_group >= 1 && topk_group <= n_group,
+                "%s: bad n_group=%d / topk_group=%d for E=%d", who, n_group, topk_group, E);
+  const int gs = E / n_group;
+  XTB_CHECK_ARG((gs & (gs - 1)) == 0 && gs % (E / 32) == 0,
+                "%s: group size %d must be a power of two and a multiple of E/32=%d", who, gs, E / 32);
+  XTB_CHECK_ARG(n_group == topk_group || gs >= 2,
+                "%s: a group mask (topk_group=%d < n_group=%d) needs at least 2 experts per group, got %d", who,
+                topk_group, n_group, gs);
+  return XTB_OK;
+}
+
 static int router_noaux_impl(const float* logits, const float* e_score_correction_bias, int T, int E, int K,
                              int n_group, int topk_group, int norm_topk_prob, float scaling, float* router_weights,
                              float* topk_weights, int64_t* topk_ids, int32_t* topk_ids_i32,
@@ -941,38 +952,24 @@ static int router_noaux_impl(const float* logits, const float* e_score_correctio
                     tokens_per_expert_f32,
                 "xtb_router_noaux: null pointer");
   XTB_CHECK_ARG(T >= 0 && E > 0 && K > 0 && K <= 32 && K <= E, "xtb_router_noaux: bad T/E/K");
-  XTB_CHECK_ARG(E % 32 == 0 && E <= 512, "xtb_router_noaux: E=%d must be a multiple of 32 and <= 512", E);
-  XTB_CHECK_ARG(n_group >= 1 && n_group <= 32 && E % n_group == 0 && topk_group >= 1 && topk_group <= n_group,
-                "xtb_router_noaux: bad n_group/topk_group");
+  if (const int rc = check_noaux_groups("xtb_router_noaux", E, n_group, topk_group)) return rc;
   XTB_ENSURE_CTX(logits);
-  const int vpl = E / 32;
-  XTB_CHECK_ARG((E / n_group) % vpl == 0, "xtb_router_noaux: group size %d must be a multiple of E/32=%d",
-                E / n_group, vpl);
-  const int lpg = (E / n_group) / vpl;
-  XTB_CHECK_ARG((lpg & (lpg - 1)) == 0, "xtb_router_noaux: lanes per group must be a power of two");
   cudaStream_t st = as_stream(stream);
   XTB_CUDA(cudaMemsetAsync(tokens_per_expert_f32, 0, sizeof(float) * E, st));
   if (T == 0) return XTB_OK;
   const int blocks = (T + 7) / 8;
 #define XTB_NOAUX(V)                                                                                                  \
-  if (replay_ids) {                                                                                                   \
-    XTB_CUDA(launch_pdl(router_noaux_kernel<V, true>, dim3(blocks), dim3(256), E * sizeof(int), st, logits,           \
-                        e_score_correction_bias, T, E, K, n_group, topk_group, norm_topk_prob, scaling,               \
-                        router_weights, topk_weights, topk_ids, topk_ids_i32, tokens_per_expert_f32, replay_ids,      \
-                        replay_stride));                                                                              \
-  } else {                                                                                                            \
-    router_noaux_kernel<V><<<blocks, 256, E * sizeof(int), st>>>(logits, e_score_correction_bias, T, E, K, n_group,   \
-                                                                 topk_group, norm_topk_prob, scaling,                 \
-                                                                 router_weights, topk_weights, topk_ids,              \
-                                                                 topk_ids_i32, tokens_per_expert_f32);                \
-  }
-  switch (vpl) {
+  XTB_CUDA(launch_pdl(replay_ids ? router_noaux_kernel<V, true> : router_noaux_kernel<V>, dim3(blocks), dim3(256),    \
+                      E * sizeof(int), st, logits, e_score_correction_bias, T, E, K, n_group, topk_group,             \
+                      norm_topk_prob, scaling, router_weights, topk_weights, topk_ids, topk_ids_i32,                  \
+                      tokens_per_expert_f32, replay_ids, replay_stride))
+  switch (E / 32) {
     case 1: XTB_NOAUX(1); break;
     case 2: XTB_NOAUX(2); break;
     case 4: XTB_NOAUX(4); break;
     case 8: XTB_NOAUX(8); break;
     case 16: XTB_NOAUX(16); break;
-    default: return fail(XTB_ERR_INVALID, "xtb_router_noaux: E/32=%d unsupported (1,2,4,8,16)", vpl);
+    default: return fail(XTB_ERR_INVALID, "xtb_router_noaux: E/32=%d unsupported (1,2,4,8,16)", E / 32);
   }
 #undef XTB_NOAUX
   XTB_LAUNCH_OK();
@@ -1018,13 +1015,10 @@ extern "C" int xtb_router_noaux_bwd(const float* logits, const float* e_score_co
   // group_spec = XTB_NOAUX_GROUP_SPEC(n_group, topk_group); 0: no group mask
   const int n_group = group_spec ? (group_spec & 0xFF) : 1;
   const int topk_group = group_spec ? (group_spec >> 8) : 1;
-  if (group_spec) {  // the forward's geometry (xtb_router_noaux): every group lies in one lane or spans 2^i lanes
-    XTB_CHECK_ARG(E % 32 == 0 && E <= 512, "xtb_router_noaux_bwd: E=%d must be a multiple of 32 and <= 512", E);
-    XTB_CHECK_ARG(n_group >= 1 && n_group <= 32 && E % n_group == 0 && topk_group >= 1 && topk_group < n_group,
-                  "xtb_router_noaux_bwd: bad group_spec %d (n_group=%d, topk_group=%d)", group_spec, n_group, topk_group);
-    XTB_CHECK_ARG(((E / n_group) & (E / n_group - 1)) == 0 && (E / n_group) % (E / 32) == 0,
-                  "xtb_router_noaux_bwd: group size %d must be a power of two and a multiple of E/32=%d", E / n_group,
-                  E / 32);
+  if (group_spec) {  // a group mask, in the forward's geometry
+    XTB_CHECK_ARG(topk_group < n_group, "xtb_router_noaux_bwd: group_spec %d is not a group mask (n_group=%d, "
+                  "topk_group=%d)", group_spec, n_group, topk_group);
+    if (const int rc = check_noaux_groups("xtb_router_noaux_bwd", E, n_group, topk_group)) return rc;
   }
   XTB_ENSURE_CTX(logits);
   if (T == 0) return XTB_OK;
