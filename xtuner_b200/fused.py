@@ -93,6 +93,24 @@ def _router_gate_bwd(lib, rw, tw, ids, g_tw, g_rw, g_lg, x, gate_w, T, H, E, K, 
     return g_gate_w, g_x_gate
 
 
+def _no_tokens(ctx, x: Tensor, gate_w: Tensor, K: int):
+    """Forward outputs of a node given no tokens (T = 0), with no launch: the kernels take no null pointers, and an empty
+    tensor has none.  Its backward returns empty / zero gradients (:func:`_no_token_grads`)."""
+    ctx.no_tokens = True
+    E, dev = gate_w.shape[0], x.device
+    ids = torch.empty((0, K), dtype=torch.int64, device=dev)
+    tpe = torch.zeros((E,), dtype=torch.int64, device=dev)
+    ctx.mark_non_differentiable(ids, tpe)
+    lg = torch.empty((0, E), dtype=torch.float32, device=dev)
+    return torch.empty_like(x), lg, lg.clone(), ids, tpe
+
+
+def _no_token_grads(gate_w: Tensor, w13: Tensor, w2: Tensor):
+    """(g_gate_w, g_w13, g_w2) of a node given no tokens: zeros, the expert ones in the GRAD_SINK buffers if set."""
+    g_w13, g_w2 = _weight_grad_buffers(w13, w2)
+    return torch.zeros_like(gate_w), g_w13.zero_(), g_w2.zero_()
+
+
 # Optional profiling: when a list, every kernel call is bracketed by CUDA events on the current stream
 # and (name, start, end) is appended.  bench.py uses this to time kernels inside the timed region.
 PROFILE: Optional[list] = None
@@ -124,6 +142,10 @@ class FusedMoEFunction(torch.autograd.Function):
         dev = x.device
         bf = torch.bfloat16
 
+        if T == 0:
+            ctx.save_for_backward(gate_w, w13, w2)
+            ctx.has_res = residual is not None
+            return _no_tokens(ctx, x, gate_w, K)
         logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st,
                                                           rollout_routed_experts)
 
@@ -148,6 +170,9 @@ class FusedMoEFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_out, g_logits, g_rw, _g_ids, _g_tpe):
+        if getattr(ctx, "no_tokens", False):
+            return (torch.empty_like(g_out), g_out if ctx.has_res else None, *_no_token_grads(*ctx.saved_tensors),
+                    None, None, None, None, None, None)
         lib = _capi.ensure_init()
         st = current_stream()
         x, gate_w, w13, w2, rw, tw, ids, row_id_map, tpe, x_perm, h, a, y = ctx.saved_tensors
@@ -207,6 +232,9 @@ class FusedMoEBlockFunction(torch.autograd.Function):
         dev = h.device
         f32, bf = torch.float32, torch.bfloat16
 
+        if T == 0:
+            ctx.save_for_backward(norm_w, gate_w, w13, w2)
+            return _no_tokens(ctx, h, gate_w, K)
         x = torch.empty((T, H), dtype=bf, device=dev)
         rstd = torch.empty((T,), dtype=f32, device=dev)
         # the norm as its own streaming kernel: folding the gate into it (xtb_rmsnorm_gate with gate_w) is not used by
@@ -232,6 +260,11 @@ class FusedMoEBlockFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_out, g_logits, g_rw, _g_ids, _g_tpe):
+        if getattr(ctx, "no_tokens", False):
+            norm_w, gate_w, w13, w2 = ctx.saved_tensors
+            g_norm_w = torch.zeros_like(norm_w) if ctx.needs_input_grad[1] else None
+            return (torch.empty_like(g_out), g_norm_w, None, *_no_token_grads(gate_w, w13, w2), None, None, None, None,
+                    None, None)
         lib = _capi.ensure_init()
         st = current_stream()
         h, norm_w, rstd, x, gate_w, w13, w2, rw, tw, ids, row_id_map, tpe, x_perm, hh, a, y = ctx.saved_tensors
