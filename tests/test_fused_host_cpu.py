@@ -242,13 +242,24 @@ def test_route_entry_points_follow_the_shape(emu, block, E):
         out, logits, rw, ids, tpe = fused.FusedMoEBlockFunction.apply(ho, norm_w, eps, go, w13, w2, K, True, 1.0, 1.0, 0)
     else:
         out, logits, rw, ids, tpe = fused.FusedMoEFunction.apply(ho, None, go, w13, w2, K, True, 1.0, 1.0, 0)
+    fwd = list(emu.calls)
     grads = torch.autograd.grad([out, rw, logits], [ho, go], [g_out, g_rw, g_lg])
+    bwd = emu.calls[len(fwd):]
 
     one_launch = {"xtb_gate_route_dispatch", "xtb_router_gate_bwd"}
     split = {"xtb_gate_logits", "xtb_router_greedy_dispatch", "xtb_router_greedy_bwd", "xtb_gate_logits_bwd"}
     called = set(emu.calls)
     want, unwanted = (one_launch, split) if E <= 8 else (split, one_launch)
     assert want <= called and not (unwanted & called), sorted(called)
+    # the launch order: the block node is the plain node with the norm ahead of it and the norm backward as its last
+    # launch in place of the dispatch backward (the emulator logs xtb_group_gemm_tn_pair after its two inner tn calls)
+    route = ["xtb_gate_route_dispatch"] if E <= 8 else ["xtb_gate_logits", "xtb_router_greedy_dispatch"]
+    route_bwd = ["xtb_router_gate_bwd"] if E <= 8 else ["xtb_router_greedy_bwd", "xtb_gate_logits_bwd"]
+    moe_fwd = route + ["xtb_moe_permute_prepared", "xtb_group_gemm_nt_swiglu", "xtb_group_gemm_nt", "xtb_moe_combine"]
+    moe_bwd = ["xtb_moe_unpermute_bwd", "xtb_group_gemm_nn", "xtb_swiglu_bwd", "xtb_group_gemm_nn", "xtb_group_gemm_tn",
+               "xtb_group_gemm_tn", "xtb_group_gemm_tn_pair"] + route_bwd
+    assert fwd == (["xtb_rmsnorm_gate"] + moe_fwd if block else moe_fwd), fwd
+    assert bwd == moe_bwd + (["xtb_moe_dispatch_bwd_rmsnorm"] if block else ["xtb_moe_combine"]), bwd
     assert torch.equal(ids, ref["router.topk_ids"]) and torch.equal(tpe, ref["tokens_per_expert"])
     _close(out, ref["hidden_states"], "hidden_states")
     torch.testing.assert_close(logits, ref["router.logits"], rtol=1e-5, atol=1e-5)

@@ -127,6 +127,74 @@ def _k(lib, name: str, *args) -> None:
     PROFILE.append((name, s, e))
 
 
+def _moe_forward(ctx, lib, st, x, residual, gate_w, w13, w2, K, norm, scaling, hidden_factor, scoring, replay):
+    """Gate and route through the combine, ``out = moe(x) * hidden_factor + residual``, for both nodes.  Returns the
+    node's outputs ``(out, logits, rw, ids, tpe)`` and the 13 tensors :func:`_moe_backward` reads, in that order."""
+    T, H = x.shape
+    E = gate_w.shape[0]
+    I = w2.shape[-1]
+    M = T * K
+    dev = x.device
+    bf = torch.bfloat16
+    logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm, scaling, st, replay)
+
+    x_perm = torch.empty((M, H), dtype=bf, device=dev)
+    row_id_map = torch.empty((M,), dtype=torch.int32, device=dev)
+    _k(lib, "xtb_moe_permute_prepared", ptr(x), ptr(ids32), T, K, E, H * 2, ptr(x_perm), ptr(row_id_map), None, ptr(ws), st)
+
+    h = torch.empty((M, 2 * I), dtype=bf, device=dev)
+    a = torch.empty((M, I), dtype=bf, device=dev)
+    _k(lib, "xtb_group_gemm_nt_swiglu", ptr(x_perm), ptr(w13), ptr(tpe), M, I, H, E, ptr(h), ptr(a), st)
+
+    y = torch.empty((M, H), dtype=bf, device=dev)
+    _k(lib, "xtb_group_gemm_nt", ptr(a), ptr(w2), ptr(tpe), M, H, I, E, ptr(y), st)
+
+    out = torch.empty((T, H), dtype=bf, device=dev)
+    _k(lib, "xtb_moe_combine", ptr(y), ptr(row_id_map), ptr(tw), ptr(residual), float(hidden_factor), T, K, H, ptr(out), st)
+
+    ctx.mark_non_differentiable(ids, tpe)
+    return (out, logits, rw, ids, tpe), (x, gate_w, w13, w2, rw, tw, ids, row_id_map, tpe, x_perm, h, a, y)
+
+
+def _moe_backward(lib, st, saved, cfg, g_out, g_logits, g_rw):
+    """From the combine backward through the router and gate backward, for both nodes: ``saved`` holds the 13 tensors
+    of :func:`_moe_forward`, ``cfg`` starts with (K, norm, scaling, hidden_factor, scoring), ``g_out`` is contiguous.
+    Returns ``(g_xp, g_x_gate, g_gate_w, g_w13, g_w2)``; the node's last launch sums each token's K rows of g_xp and
+    adds g_x_gate."""
+    x, gate_w, w13, w2, rw, tw, ids, row_id_map, tpe, x_perm, h, a, y = saved
+    K, norm, scaling, hidden_factor, scoring = cfg[:5]
+    T, H = x.shape
+    E = gate_w.shape[0]
+    I = a.shape[1]
+    M = T * K
+    dev = x.device
+    bf, f32 = torch.bfloat16, torch.float32
+    g_comb = g_out if hidden_factor == 1.0 else (g_out * hidden_factor)
+
+    g_y = torch.empty((M, H), dtype=bf, device=dev)
+    g_tw = torch.empty((T, K), dtype=f32, device=dev)
+    _k(lib, "xtb_moe_unpermute_bwd", ptr(g_comb), ptr(y), ptr(row_id_map), ptr(tw), T, K, H, ptr(g_y), ptr(g_tw), st)
+
+    g_w13, g_w2 = _weight_grad_buffers(w13, w2)
+    g_a = torch.empty((M, I), dtype=bf, device=dev)
+    _k(lib, "xtb_group_gemm_nn", ptr(g_y), ptr(w2), ptr(tpe), M, H, I, E, ptr(g_a), st)
+    g_h = torch.empty((M, 2 * I), dtype=bf, device=dev)
+    _k(lib, "xtb_swiglu_bwd", ptr(g_a), ptr(h), ptr(g_h), M, I, st)
+
+    g_xp = torch.empty((M, H), dtype=bf, device=dev)
+    _k(lib, "xtb_group_gemm_nn", ptr(g_h), ptr(w13), ptr(tpe), M, 2 * I, H, E, ptr(g_xp), st)
+    # both weight gradients in one launch: one tile list over the two products fills the persistent schedule's last wave
+    _k(lib, "xtb_group_gemm_tn_pair", ptr(g_y), ptr(a), H, I, ptr(g_w2), ptr(g_h), ptr(x_perm), 2 * I, H, ptr(g_w13),
+       ptr(tpe), M, E, st)
+
+    g_gate_w, g_x_gate = _router_gate_bwd(lib, rw, tw, ids, g_tw, g_rw, g_logits, x, gate_w, T, H, E, K, scoring, norm,
+                                          scaling, st)
+    return g_xp, g_x_gate, g_gate_w, g_w13, g_w2
+
+
+_ROW_ID_MAP = 7  # where row_id_map sits among the 13 tensors of _moe_forward: the node's last launch reads it
+
+
 class FusedMoEFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x: Tensor, residual: Optional[Tensor], gate_w: Tensor, w13: Tensor, w2: Tensor, top_k: int,
@@ -134,39 +202,15 @@ class FusedMoEFunction(torch.autograd.Function):
                 rollout_routed_experts: Optional[Tensor] = None):
         lib = _capi.ensure_init()
         st = current_stream()
-        T, H = x.shape
-        E = gate_w.shape[0]
-        I = w2.shape[1] if w2.dim() == 2 else w2.shape[2]
-        K = top_k
-        M = T * K
-        dev = x.device
-        bf = torch.bfloat16
-
-        if T == 0:
+        if x.shape[0] == 0:
             ctx.save_for_backward(gate_w, w13, w2)
             ctx.has_res = residual is not None
-            return _no_tokens(ctx, x, gate_w, K)
-        logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st,
-                                                          rollout_routed_experts)
-
-        x_perm = torch.empty((M, H), dtype=bf, device=dev)
-        row_id_map = torch.empty((M,), dtype=torch.int32, device=dev)
-        _k(lib, "xtb_moe_permute_prepared", ptr(x), ptr(ids32), T, K, E, H * 2, ptr(x_perm), ptr(row_id_map), None, ptr(ws), st)
-
-        h = torch.empty((M, 2 * I), dtype=bf, device=dev)
-        a = torch.empty((M, I), dtype=bf, device=dev)
-        _k(lib, "xtb_group_gemm_nt_swiglu", ptr(x_perm), ptr(w13), ptr(tpe), M, I, H, E, ptr(h), ptr(a), st)
-
-        y = torch.empty((M, H), dtype=bf, device=dev)
-        _k(lib, "xtb_group_gemm_nt", ptr(a), ptr(w2), ptr(tpe), M, H, I, E, ptr(y), st)
-
-        out = torch.empty((T, H), dtype=bf, device=dev)
-        _k(lib, "xtb_moe_combine", ptr(y), ptr(row_id_map), ptr(tw), ptr(residual), float(hidden_factor), T, K, H, ptr(out), st)
-
-        ctx.save_for_backward(x, gate_w, w13, w2, rw, tw, ids, row_id_map, tpe, x_perm, h, a, y)
-        ctx.cfg = (K, norm_topk_prob, scaling, hidden_factor, scoring, residual is not None)
-        ctx.mark_non_differentiable(ids, tpe)
-        return out, logits, rw, ids, tpe
+            return _no_tokens(ctx, x, gate_w, top_k)
+        outputs, saved = _moe_forward(ctx, lib, st, x, residual, gate_w, w13, w2, top_k, norm_topk_prob, scaling,
+                                      hidden_factor, scoring, rollout_routed_experts)
+        ctx.save_for_backward(*saved)
+        ctx.cfg = (top_k, norm_topk_prob, scaling, hidden_factor, scoring, residual is not None)
+        return outputs
 
     @staticmethod
     def backward(ctx, g_out, g_logits, g_rw, _g_ids, _g_tpe):
@@ -175,42 +219,16 @@ class FusedMoEFunction(torch.autograd.Function):
                     None, None, None, None, None, None)
         lib = _capi.ensure_init()
         st = current_stream()
-        x, gate_w, w13, w2, rw, tw, ids, row_id_map, tpe, x_perm, h, a, y = ctx.saved_tensors
-        K, norm, scaling, hidden_factor, scoring, has_res = ctx.cfg
-        T, H = x.shape
-        E = gate_w.shape[0]
-        I = a.shape[1]
-        M = T * K
-        dev = x.device
-        bf, f32 = torch.bfloat16, torch.float32
+        saved = ctx.saved_tensors
+        K, has_res = ctx.cfg[0], ctx.cfg[5]
         g_out = g_out.contiguous()
-        g_comb = g_out if hidden_factor == 1.0 else (g_out * hidden_factor)
-
-        g_y = torch.empty((M, H), dtype=bf, device=dev)
-        g_tw = torch.empty((T, K), dtype=f32, device=dev)
-        _k(lib, "xtb_moe_unpermute_bwd", ptr(g_comb), ptr(y), ptr(row_id_map), ptr(tw), T, K, H, ptr(g_y), ptr(g_tw), st)
-
-        g_w13, g_w2 = _weight_grad_buffers(w13, w2)
-        g_a = torch.empty((M, I), dtype=bf, device=dev)
-        _k(lib, "xtb_group_gemm_nn", ptr(g_y), ptr(w2), ptr(tpe), M, H, I, E, ptr(g_a), st)
-        g_h = torch.empty((M, 2 * I), dtype=bf, device=dev)
-        _k(lib, "xtb_swiglu_bwd", ptr(g_a), ptr(h), ptr(g_h), M, I, st)
-
-        g_xp = torch.empty((M, H), dtype=bf, device=dev)
-        _k(lib, "xtb_group_gemm_nn", ptr(g_h), ptr(w13), ptr(tpe), M, 2 * I, H, E, ptr(g_xp), st)
-        # both weight gradients in one launch: one tile list over the two products fills the persistent schedule's last wave
-        _k(lib, "xtb_group_gemm_tn_pair", ptr(g_y), ptr(a), H, I, ptr(g_w2), ptr(g_h), ptr(x_perm), 2 * I, H, ptr(g_w13),
-           ptr(tpe), M, E, st)
-
-        g_gate_w, g_x_gate = _router_gate_bwd(lib, rw, tw, ids, g_tw, g_rw, g_logits, x, gate_w, T, H, E, K, scoring, norm,
-                                              scaling, st)
+        g_xp, g_x_gate, g_gate_w, g_w13, g_w2 = _moe_backward(lib, st, saved, ctx.cfg, g_out, g_logits, g_rw)
 
         # dispatch backward (sum of the K copies' grads) fused with "+ gate-path grad" (autograd's add)
-        g_x = torch.empty((T, H), dtype=bf, device=dev)
-        _k(lib, "xtb_moe_combine", ptr(g_xp), ptr(row_id_map), None, ptr(g_x_gate), 1.0, T, K, H, ptr(g_x), st)
-
-        g_res = g_out if has_res else None
-        return g_x, g_res, g_gate_w, g_w13, g_w2, None, None, None, None, None, None
+        T, H = g_x_gate.shape
+        g_x = torch.empty_like(g_x_gate)
+        _k(lib, "xtb_moe_combine", ptr(g_xp), ptr(saved[_ROW_ID_MAP]), None, ptr(g_x_gate), 1.0, T, K, H, ptr(g_x), st)
+        return g_x, g_out if has_res else None, g_gate_w, g_w13, g_w2, None, None, None, None, None, None
 
 
 class FusedMoEBlockFunction(torch.autograd.Function):
@@ -225,38 +243,20 @@ class FusedMoEBlockFunction(torch.autograd.Function):
         lib = _capi.ensure_init()
         st = current_stream()
         T, H = h.shape
-        E = gate_w.shape[0]
-        I = w2.shape[1] if w2.dim() == 2 else w2.shape[2]
-        K = top_k
-        M = T * K
-        dev = h.device
-        f32, bf = torch.float32, torch.bfloat16
-
         if T == 0:
             ctx.save_for_backward(norm_w, gate_w, w13, w2)
-            return _no_tokens(ctx, h, gate_w, K)
-        x = torch.empty((T, H), dtype=bf, device=dev)
-        rstd = torch.empty((T,), dtype=f32, device=dev)
+            return _no_tokens(ctx, h, gate_w, top_k)
+        E = gate_w.shape[0]
+        x = torch.empty((T, H), dtype=torch.bfloat16, device=h.device)
+        rstd = torch.empty((T,), dtype=torch.float32, device=h.device)
         # the norm as its own streaming kernel: folding the gate into it (xtb_rmsnorm_gate with gate_w) is not used by
         # the fused layer (not measured on H100)
         _k(lib, "xtb_rmsnorm_gate", ptr(h), ptr(norm_w), None, float(eps), T, H, E, ptr(x), ptr(rstd), None, st)
-        logits, rw, tw, ids, ids32, tpe, ws = _gate_route(lib, x, gate_w, T, H, E, K, scoring, norm_topk_prob, scaling, st,
-                                                          rollout_routed_experts)
-        x_perm = torch.empty((M, H), dtype=bf, device=dev)
-        row_id_map = torch.empty((M,), dtype=torch.int32, device=dev)
-        _k(lib, "xtb_moe_permute_prepared", ptr(x), ptr(ids32), T, K, E, H * 2, ptr(x_perm), ptr(row_id_map), None, ptr(ws), st)
-        hh = torch.empty((M, 2 * I), dtype=bf, device=dev)
-        a = torch.empty((M, I), dtype=bf, device=dev)
-        _k(lib, "xtb_group_gemm_nt_swiglu", ptr(x_perm), ptr(w13), ptr(tpe), M, I, H, E, ptr(hh), ptr(a), st)
-        y = torch.empty((M, H), dtype=bf, device=dev)
-        _k(lib, "xtb_group_gemm_nt", ptr(a), ptr(w2), ptr(tpe), M, H, I, E, ptr(y), st)
-        out = torch.empty((T, H), dtype=bf, device=dev)
-        _k(lib, "xtb_moe_combine", ptr(y), ptr(row_id_map), ptr(tw), ptr(h), float(hidden_factor), T, K, H, ptr(out), st)
-
-        ctx.save_for_backward(h, norm_w, rstd, x, gate_w, w13, w2, rw, tw, ids, row_id_map, tpe, x_perm, hh, a, y)
-        ctx.cfg = (K, norm_topk_prob, scaling, hidden_factor, scoring)
-        ctx.mark_non_differentiable(ids, tpe)
-        return out, logits, rw, ids, tpe
+        outputs, saved = _moe_forward(ctx, lib, st, x, h, gate_w, w13, w2, top_k, norm_topk_prob, scaling, hidden_factor,
+                                      scoring, rollout_routed_experts)
+        ctx.save_for_backward(h, norm_w, rstd, *saved)
+        ctx.cfg = (top_k, norm_topk_prob, scaling, hidden_factor, scoring)
+        return outputs
 
     @staticmethod
     def backward(ctx, g_out, g_logits, g_rw, _g_ids, _g_tpe):
@@ -267,44 +267,37 @@ class FusedMoEBlockFunction(torch.autograd.Function):
                     None, None)
         lib = _capi.ensure_init()
         st = current_stream()
-        h, norm_w, rstd, x, gate_w, w13, w2, rw, tw, ids, row_id_map, tpe, x_perm, hh, a, y = ctx.saved_tensors
-        K, norm, scaling, hidden_factor, scoring = ctx.cfg
-        T, H = h.shape
-        E = gate_w.shape[0]
-        I = a.shape[1]
-        M = T * K
-        dev = h.device
-        bf, f32 = torch.bfloat16, torch.float32
+        h, norm_w, rstd, *saved = ctx.saved_tensors
+        K = ctx.cfg[0]
         g_out = g_out.contiguous()
-        g_comb = g_out if hidden_factor == 1.0 else (g_out * hidden_factor)
+        g_xp, g_x_gate, g_gate_w, g_w13, g_w2 = _moe_backward(lib, st, saved, ctx.cfg, g_out, g_logits, g_rw)
 
-        g_y = torch.empty((M, H), dtype=bf, device=dev)
-        g_tw = torch.empty((T, K), dtype=f32, device=dev)
-        _k(lib, "xtb_moe_unpermute_bwd", ptr(g_comb), ptr(y), ptr(row_id_map), ptr(tw), T, K, H, ptr(g_y), ptr(g_tw), st)
-        g_w13, g_w2 = _weight_grad_buffers(w13, w2)
-        g_a = torch.empty((M, I), dtype=bf, device=dev)
-        _k(lib, "xtb_group_gemm_nn", ptr(g_y), ptr(w2), ptr(tpe), M, H, I, E, ptr(g_a), st)
-        g_h2 = torch.empty((M, 2 * I), dtype=bf, device=dev)
-        _k(lib, "xtb_swiglu_bwd", ptr(g_a), ptr(hh), ptr(g_h2), M, I, st)
-        g_xp = torch.empty((M, H), dtype=bf, device=dev)
-        _k(lib, "xtb_group_gemm_nn", ptr(g_h2), ptr(w13), ptr(tpe), M, 2 * I, H, E, ptr(g_xp), st)
-        # both weight gradients in one launch: one tile list over the two products fills the persistent schedule's last wave
-        _k(lib, "xtb_group_gemm_tn_pair", ptr(g_y), ptr(a), H, I, ptr(g_w2), ptr(g_h2), ptr(x_perm), 2 * I, H, ptr(g_w13),
-           ptr(tpe), M, E, st)
-
-        g_gate_w, g_x_gate = _router_gate_bwd(lib, rw, tw, ids, g_tw, g_rw, g_logits, x, gate_w, T, H, E, K, scoring, norm,
-                                              scaling, st)
-
-        g_h = torch.empty((T, H), dtype=bf, device=dev)
-        need_nw = ctx.needs_input_grad[1]
-        g_norm_w = torch.empty_like(norm_w) if need_nw else None
-        wsn = ops._scratch("norm_bwd", int(lib.xtb_moe_dispatch_bwd_rmsnorm_workspace_bytes(T, H)), dev) if need_nw else None
-        _k(lib, "xtb_moe_dispatch_bwd_rmsnorm", ptr(g_xp), ptr(row_id_map), ptr(g_x_gate), ptr(h), ptr(rstd), ptr(norm_w),
-           ptr(g_out), T, K, H, ptr(g_h), ptr(g_norm_w), ptr(wsn), st)
+        T, H = h.shape
+        g_h = torch.empty_like(g_x_gate)
+        g_norm_w = wsn = None
+        if ctx.needs_input_grad[1]:
+            g_norm_w = torch.empty_like(norm_w)
+            wsn = ops._scratch("norm_bwd", int(lib.xtb_moe_dispatch_bwd_rmsnorm_workspace_bytes(T, H)), h.device)
+        _k(lib, "xtb_moe_dispatch_bwd_rmsnorm", ptr(g_xp), ptr(saved[_ROW_ID_MAP]), ptr(g_x_gate), ptr(h), ptr(rstd),
+           ptr(norm_w), ptr(g_out), T, K, H, ptr(g_h), ptr(g_norm_w), ptr(wsn), st)
         return g_h, g_norm_w, None, g_gate_w, g_w13, g_w2, None, None, None, None, None, None
 
 
 _FUSED_NORM_H = (256, 512, 1024, 2048)
+
+
+def _fp32_gate(entry: str, x: Tensor, gate_weight: Tensor, w13: Tensor, w2: Tensor) -> Tensor:
+    """The gate weight in fp32, once ``entry``'s activations and expert weights have passed its checks."""
+    if not x.is_cuda:
+        raise _capi.XtbError(f"{entry} needs CUDA tensors (no CPU fallback)")
+    if x.dtype != torch.bfloat16 or w13.dtype != torch.bfloat16 or w2.dtype != torch.bfloat16:
+        raise TypeError(f"{entry}: activations and expert weights must be bfloat16")
+    return gate_weight if gate_weight.dtype == torch.float32 else gate_weight.float()
+
+
+def _router_results(logits: Tensor, rw: Tensor, ids: Tensor, tpe: Tensor) -> dict:
+    """The reference's RouterResults of a fused node (topk_weights stay inside the node)."""
+    return {"logits": logits, "router_weights": rw, "topk_weights": None, "topk_ids": ids, "topkens_per_expert": tpe}
 
 
 def fused_moe_block(h: Tensor, norm_weight: Tensor, eps: float, gate_weight: Tensor, w13: Tensor, w2: Tensor, *, top_k: int,
@@ -313,25 +306,20 @@ def fused_moe_block(h: Tensor, norm_weight: Tensor, eps: float, gate_weight: Ten
     """``h`` [T,H] bf16 residual stream -> ``moe(rms_norm(h, norm_weight, eps)) * hidden_factor + h``.
     Supported H for the fused backward: 256/512/1024/2048.  ``rollout_routed_experts`` (int64 [T, top_k], on h's device):
     route those experts instead of the router's top-k (RL routing replay).  Returns ``(hidden_states, router_results)``."""
-    if not h.is_cuda:
-        raise _capi.XtbError("fused_moe_block needs CUDA tensors (no CPU fallback)")
-    if h.dtype != torch.bfloat16 or w13.dtype != torch.bfloat16 or w2.dtype != torch.bfloat16:
-        raise TypeError("fused_moe_block: activations and expert weights must be bfloat16")
+    gw = _fp32_gate("fused_moe_block", h, gate_weight, w13, w2)
     shape = h.shape
     if shape[-1] not in _FUSED_NORM_H:
         # the fused norm kernels keep the row slice in registers (xtb_rmsnorm_gate: H in 256/512/1024/2048): compose instead
         x = torch.nn.functional.rms_norm(h, (shape[-1],), norm_weight.to(h.dtype), eps)
-        return fused_moe(x, h, gate_weight, w13, w2, top_k=top_k, norm_topk_prob=norm_topk_prob,
+        return fused_moe(x, h, gw, w13, w2, top_k=top_k, norm_topk_prob=norm_topk_prob,
                          router_scaling_factor=router_scaling_factor, hidden_factor=hidden_factor, scoring_func=scoring_func,
                          rollout_routed_experts=rollout_routed_experts)
     h2 = h.contiguous().view(-1, shape[-1])
-    gw = gate_weight if gate_weight.dtype == torch.float32 else gate_weight.float()
     nw = norm_weight if norm_weight.dtype == torch.float32 else norm_weight.float()
-    out, logits, rw, ids, tpe = FusedMoEBlockFunction.apply(
+    out, *rr = FusedMoEBlockFunction.apply(
         h2, nw.contiguous(), eps, gw.contiguous(), w13.contiguous(), w2.contiguous(), top_k, norm_topk_prob,
         router_scaling_factor, hidden_factor, SCORING[scoring_func], rollout_routed_experts)
-    rr = {"logits": logits, "router_weights": rw, "topk_weights": None, "topk_ids": ids, "topkens_per_expert": tpe}
-    return out.view(shape), rr
+    return out.view(shape), _router_results(*rr)
 
 
 def fused_moe(x: Tensor, residual: Optional[Tensor], gate_weight: Tensor, w13: Tensor, w2: Tensor, *, top_k: int,
@@ -341,19 +329,29 @@ def fused_moe(x: Tensor, residual: Optional[Tensor], gate_weight: Tensor, w13: T
     ``gate_weight`` [E,H] (used in fp32), ``w13`` [E*2I,H] or [E,2I,H], ``w2`` [E*H,I] or [E,H,I] (bf16),
     ``rollout_routed_experts`` int64 [T, top_k] or None (RL routing replay, as in :func:`fused_moe_block`).
     Returns ``(hidden_states, router_results)`` with the reference's RouterResults keys."""
-    if not x.is_cuda:
-        raise _capi.XtbError("fused_moe needs CUDA tensors (no CPU fallback)")
-    if x.dtype != torch.bfloat16 or w13.dtype != torch.bfloat16 or w2.dtype != torch.bfloat16:
-        raise TypeError("fused_moe: activations and expert weights must be bfloat16")
+    gw = _fp32_gate("fused_moe", x, gate_weight, w13, w2)
     shape = x.shape
     x2 = x.contiguous().view(-1, shape[-1])
     res2 = None if residual is None else residual.contiguous().view(-1, shape[-1])
-    gw = gate_weight if gate_weight.dtype == torch.float32 else gate_weight.float()
-    out, logits, rw, ids, tpe = FusedMoEFunction.apply(
+    out, *rr = FusedMoEFunction.apply(
         x2, res2, gw.contiguous(), w13.contiguous(), w2.contiguous(), top_k, norm_topk_prob, router_scaling_factor,
         hidden_factor, SCORING[scoring_func], rollout_routed_experts)
-    rr = {"logits": logits, "router_weights": rw, "topk_weights": None, "topk_ids": ids, "topkens_per_expert": tpe}
-    return out.view(shape), rr
+    return out.view(shape), _router_results(*rr)
+
+
+def _add_gate_and_experts(mod: nn.Module, hidden_size: int, moe_intermediate_size: int, n_routed_experts: int,
+                          num_experts_per_tok: int, norm_topk_prob: bool, router_scaling_factor: float,
+                          hidden_factor: float) -> None:
+    """The routing settings and the ``gate`` / ``experts`` submodules both fused modules register, named as in
+    :class:`xtuner_b200.moe.MoELayer`."""
+    from .moe import MoEBlock, MoEGate
+
+    mod.top_k, mod.norm_topk_prob = num_experts_per_tok, norm_topk_prob
+    mod.router_scaling_factor, mod.hidden_factor = router_scaling_factor, hidden_factor
+    mod.gate = MoEGate(hidden_size=hidden_size, n_routed_experts=n_routed_experts, num_experts_per_tok=num_experts_per_tok,
+                       norm_topk_prob=norm_topk_prob, router_scaling_factor=router_scaling_factor)
+    mod.experts = MoEBlock(hidden_size=hidden_size, moe_intermediate_size=moe_intermediate_size,
+                           n_routed_experts=n_routed_experts)
 
 
 class FusedMoEBlock(nn.Module):
@@ -364,16 +362,11 @@ class FusedMoEBlock(nn.Module):
                  rms_norm_eps: float = 1e-6, norm_topk_prob: bool = True, router_scaling_factor: float = 1.0,
                  hidden_factor: float = 1.0):
         super().__init__()
-        from .moe import MoEBlock, MoEGate
-
-        self.top_k, self.eps = num_experts_per_tok, rms_norm_eps
-        self.norm_topk_prob, self.router_scaling_factor, self.hidden_factor = norm_topk_prob, router_scaling_factor, hidden_factor
+        self.eps = rms_norm_eps
         self.post_attention_layernorm = nn.Module()
         self.post_attention_layernorm.weight = nn.Parameter(torch.ones(hidden_size))
-        self.gate = MoEGate(hidden_size=hidden_size, n_routed_experts=n_routed_experts, num_experts_per_tok=num_experts_per_tok,
-                            norm_topk_prob=norm_topk_prob, router_scaling_factor=router_scaling_factor)
-        self.experts = MoEBlock(hidden_size=hidden_size, moe_intermediate_size=moe_intermediate_size,
-                                n_routed_experts=n_routed_experts)
+        _add_gate_and_experts(self, hidden_size, moe_intermediate_size, n_routed_experts, num_experts_per_tok,
+                              norm_topk_prob, router_scaling_factor, hidden_factor)
 
     def forward(self, hidden_states: Tensor):
         return fused_moe_block(hidden_states, self.post_attention_layernorm.weight, self.eps, self.gate.weight,
@@ -389,16 +382,8 @@ class FusedMoELayer(nn.Module):
     def __init__(self, *, hidden_size: int, moe_intermediate_size: int, n_routed_experts: int, num_experts_per_tok: int,
                  norm_topk_prob: bool = True, router_scaling_factor: float = 1.0, hidden_factor: float = 1.0):
         super().__init__()
-        from .moe import MoEBlock, MoEGate
-
-        self.top_k = num_experts_per_tok
-        self.norm_topk_prob = norm_topk_prob
-        self.router_scaling_factor = router_scaling_factor
-        self.hidden_factor = hidden_factor
-        self.gate = MoEGate(hidden_size=hidden_size, n_routed_experts=n_routed_experts, num_experts_per_tok=num_experts_per_tok,
-                            norm_topk_prob=norm_topk_prob, router_scaling_factor=router_scaling_factor)
-        self.experts = MoEBlock(hidden_size=hidden_size, moe_intermediate_size=moe_intermediate_size,
-                                n_routed_experts=n_routed_experts)
+        _add_gate_and_experts(self, hidden_size, moe_intermediate_size, n_routed_experts, num_experts_per_tok,
+                              norm_topk_prob, router_scaling_factor, hidden_factor)
 
     def forward(self, hidden_states: Tensor, residual: Tensor | None = None):
         return fused_moe(hidden_states, residual, self.gate.weight, self.experts.fused_w1w3.weight,
