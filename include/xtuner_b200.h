@@ -270,6 +270,30 @@ size_t xtb_lm_head_ce_workspace_bytes(int64_t T, int V);
 int xtb_lm_head_ce(const void* h, const void* w, const int64_t* labels, const float* loss_weight, int64_t T, int H, int V,
                    int64_t ignore_index, int need_grad, void* z_or_G, void* workspace, float* row_ce, float* loss, void* dh,
                    void* dW, xtb_stream_t stream);
+/* ---- f5  lm_head label log-probabilities: rl/utils/misc.py gather_logprobs(F.linear(h, W).float(), labels), the call of
+ * loss/rl_loss.py LogProbContext.loss_fn and of rl/loss/grpo_loss.py GRPOLossContext.loss_fn, split around logp so that
+ * any per-token loss of logp runs between the two entries.  For T rows of h[T,H] (bf16), head weight w[V,H] (bf16, no
+ * bias) and labels[T] (int64), with lab_t = max(labels[t], 0) (gather_logprobs clips: an ignored -100 reads token 0):
+ *   z           = bf16(h . w^T), fp32 accumulation                                  ([T,V] bf16, in z)
+ *   lsm         = (z - max) - log(sum exp(z - max))  per row, fp32 (torch's log_softmax)
+ *   logp[t]     = lsm[t, lab_t]                       (fp32 [T]; -logp[t] equals xtb_lm_head_ce's row_ce[t] bit for bit
+ *                                                      wherever that row is not ignored there)
+ *   row_stats   = (max, log sum) per row              (fp32 [T,2], 8-byte aligned; NULL to skip)
+ * The row pass reads the per-tile pairs of the logits epilogue and one logit per row.  lab_t >= V does not fault: that
+ * row's logp and log sum are NaN.  T == 0 writes nothing.  workspace: xtb_lm_head_logprob_workspace_bytes(T, V) bytes,
+ * 16-byte aligned, no initialisation needed. */
+size_t xtb_lm_head_logprob_workspace_bytes(int64_t T, int V);
+int xtb_lm_head_logprob(const void* h, const void* w, const int64_t* labels, int64_t T, int H, int V, void* z,
+                        void* workspace, float* logp, float* row_stats, xtb_stream_t stream);
+/* The backward for grad_logp[t] = c_t = dL/dlogp[t] (fp32 [T]), with z and row_stats of the forward above:
+ *   G    = bf16([v == lab_t] * c_t - exp(lsm_v) * c_t), written OVER z in z_or_G (torch's log_softmax backward of gather's
+ *          scatter; rounded as xtb_lm_head_ce rounds its G: with c_t = -loss_weight[t] the two G are equal bit for bit)
+ *   dh[T,H] = bf16(G . w),  dW[V,H] = bf16(G^T . h)   (fp32 accumulation; the NN / TN grouped GEMMs with one group)
+ * z is consumed: a second call on the same buffer reads G, not z.  T == 0 writes dW = 0.  workspace: at least
+ * xtb_lm_head_logprob_workspace_bytes(0, V) bytes, 16-byte aligned. */
+int xtb_lm_head_logprob_bwd(void* z_or_G, const float* row_stats, const int64_t* labels, const float* grad_logp,
+                            const void* h, const void* w, int64_t T, int H, int V, void* workspace, void* dh, void* dW,
+                            xtb_stream_t stream);
 /* ---- a8  native_swiglu: ops/act_fn.py:7-9 ---------------------------------------------------------
  * out[m, j] = bf16( bf16(silu(h[m, j])) * h[m, I + j] ),  h is [M, 2I] bf16 (gate | up).  I % 8 == 0; every pointer of
  * both entries 16-byte aligned. */

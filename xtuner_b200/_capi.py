@@ -144,6 +144,14 @@ SIGNATURES = {
         [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
          c_void_p, c_void_p, c_void_p],
     ),
+    "xtb_lm_head_logprob_workspace_bytes": (c_size_t, [c_int64, c_int]),
+    "xtb_lm_head_logprob": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "xtb_lm_head_logprob_bwd": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
+         c_void_p],
+    ),
     "xtb_swiglu": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "xtb_swiglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
 }

@@ -21,7 +21,7 @@ from . import _capi
 from ._capi import check, current_stream, ptr
 
 __all__ = ["permute", "unpermute", "group_gemm", "swiglu", "gate_logits", "permute_workspace", "lm_head_cross_entropy",
-           "qk_norm_rope"]
+           "lm_head_logprobs", "qk_norm_rope"]
 
 
 def _require_cuda(*tensors: Tensor) -> None:
@@ -521,6 +521,92 @@ def lm_head_cross_entropy(hidden: Tensor, weight: Tensor, labels: Tensor, loss_w
         raise ValueError(f"lm_head_cross_entropy: chunk_size must be positive (got {chunk_size})")
     need_grad = torch.is_grad_enabled() and (hidden.requires_grad or weight.requires_grad)
     return _LMHeadCrossEntropy.apply(h, weight.contiguous(), lab, lw, int(ignore_index), chunk_size, need_grad)
+
+
+# ======================================================================================================
+# lm_head label log-probabilities (f5): gather_logprobs(F.linear(h, W).float(), labels) of LogProbContext and
+# GRPOLossContext, with the per-token loss of logp left to torch
+# ======================================================================================================
+
+
+def _lm_head_logprob_call(h, w, labels, z, logp, row_stats) -> None:
+    lib = _capi.ensure_init()
+    T, H = h.shape
+    V = w.shape[0]
+    ws = _scratch("lm_head_logprob", int(lib.xtb_lm_head_logprob_workspace_bytes(T, V)), h.device)
+    check(lib.xtb_lm_head_logprob(ptr(h), ptr(w), ptr(labels), T, H, V, ptr(z), ptr(ws), ptr(logp), ptr(row_stats),
+                                  current_stream()), "xtb_lm_head_logprob")
+
+
+class _LMHeadLogProbs(torch.autograd.Function):
+    """One node over all rows: the forward keeps z ([T, V] bf16) and the row statistics, the backward writes G over z from
+    ``dL/dlogp`` and returns dh and dW.  G replaces z, so the node can be differentiated once."""
+
+    @staticmethod
+    def forward(ctx, h: Tensor, w: Tensor, labels: Tensor):
+        T, V = h.shape[0], w.shape[0]
+        z = torch.empty((T, V), dtype=torch.bfloat16, device=h.device)
+        logp = torch.empty((T,), dtype=torch.float32, device=h.device)
+        row_stats = torch.empty((T, 2), dtype=torch.float32, device=h.device)
+        if T:  # an empty tensor has no address, which the entries reject
+            _lm_head_logprob_call(h, w, labels, z, logp, row_stats)
+        ctx.save_for_backward(z, row_stats, labels, h, w)
+        ctx.consumed = False
+        return logp
+
+    @staticmethod
+    def backward(ctx, grad_logp):
+        if ctx.consumed:
+            raise RuntimeError("lm_head_logprobs: the backward overwrites the saved logits with their gradient, so it runs "
+                               "once per forward; recompute the forward instead of backpropagating twice")
+        ctx.consumed = True
+        z, row_stats, labels, h, w = ctx.saved_tensors
+        T, H = h.shape
+        V = w.shape[0]
+        if T == 0:
+            return (torch.empty_like(h) if ctx.needs_input_grad[0] else None,
+                    torch.zeros_like(w) if ctx.needs_input_grad[1] else None, None)
+        g = grad_logp.to(torch.float32).contiguous()
+        dh, dw = torch.empty_like(h), torch.empty_like(w)
+        lib = _capi.ensure_init()
+        ws = _scratch("lm_head_logprob", int(lib.xtb_lm_head_logprob_workspace_bytes(0, V)), h.device)
+        check(lib.xtb_lm_head_logprob_bwd(ptr(z), ptr(row_stats), ptr(labels), ptr(g), ptr(h), ptr(w), T, H, V, ptr(ws),
+                                          ptr(dh), ptr(dw), current_stream()), "xtb_lm_head_logprob_bwd")
+        return (dh if ctx.needs_input_grad[0] else None, dw if ctx.needs_input_grad[1] else None, None)
+
+
+def lm_head_logprobs(hidden: Tensor, weight: Tensor, labels: Tensor, chunk_size: int | None = None) -> Tensor:
+    """``gather_logprobs(F.linear(hidden, weight).float(), labels)`` (rl/utils/misc.py): the fp32 log-probability of each
+    row's label under the bf16 logits, shaped like ``labels``.  Labels are clipped at 0 as there, so an ignored position
+    (-100) gets the log-probability of token 0; a label ``>= V`` gives NaN in its row.  ``hidden`` is ``[..., H]`` bf16,
+    ``weight`` ``[V, H]`` bf16 with ``V % 128 == 0`` and ``H % 128 == 0``, ``labels`` holds one entry per row.
+
+    Without grad (grad mode off, or neither ``hidden`` nor ``weight`` requires it) the forward runs ``chunk_size`` rows at
+    a time (all at once for None) through one reused ``[chunk_size, V]`` bf16 buffer; rows are independent, so the result
+    does not depend on ``chunk_size``.  With grad it is one autograd node that keeps the ``[rows, V]`` bf16 logits for its
+    backward, which overwrites them: a second backward through the same call raises."""
+    _require_cuda(hidden, weight, labels)
+    _bf16(hidden, "hidden")
+    _bf16(weight, "weight")
+    if weight.dim() != 2 or hidden.shape[-1] != weight.shape[1]:
+        raise _capi.XtbError(f"lm_head_logprobs: weight must be [V, {hidden.shape[-1]}] (got {tuple(weight.shape)})")
+    h = hidden.reshape(-1, hidden.shape[-1]).contiguous()
+    lab = labels.reshape(-1).to(torch.int64).contiguous()
+    if lab.numel() != h.shape[0]:
+        raise _capi.XtbError(f"lm_head_logprobs: {h.shape[0]} rows but {lab.numel()} labels")
+    if chunk_size is not None and chunk_size <= 0:
+        raise ValueError(f"lm_head_logprobs: chunk_size must be positive (got {chunk_size})")
+    w = weight.contiguous()
+    if torch.is_grad_enabled() and (hidden.requires_grad or weight.requires_grad):
+        return _LMHeadLogProbs.apply(h, w, lab).view(labels.shape)
+    T = h.shape[0]
+    step = max(T, 1) if chunk_size is None else chunk_size
+    z = torch.empty((min(step, T), w.shape[0]), dtype=torch.bfloat16, device=h.device)
+    logp = torch.empty((T,), dtype=torch.float32, device=h.device)
+    for s in range(0, T, step):
+        n = min(step, T - s)
+        _lm_head_logprob_call(h[s:s + n], w, lab[s:s + n], z[:n], logp[s:s + n], None)
+    return logp.view(labels.shape)
 
 
 # ======================================================================================================

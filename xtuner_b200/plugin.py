@@ -17,9 +17,10 @@ routing replay) included; the per-op classes above stay installed for the path t
 (micro-batched forward).
 
 Everything else of the model (attention, norms, lm_head, FSDP wrapping, checkpoint keys) is untouched;
-``install_lm_head_loss()`` separately moves the lm_head cross-entropy onto this package's kernels, and
-``install_qk_norm_rope(model)`` the q/k norm and rotary embedding in front of the attention; parameters keep
-their names, so state dicts and DCP checkpoints stay compatible.  ``restore_model`` undoes the conversion.
+``install_lm_head_loss()`` separately moves the lm_head cross-entropy onto this package's kernels,
+``install_rl_lm_head()`` the RL trainer's lm_head log-probabilities and GRPO loss, and
+``install_qk_norm_rope(model)`` the q/k norm and rotary embedding in front of the attention; parameters keep their
+names, so state dicts and DCP checkpoints stay compatible.  ``restore_model`` undoes the conversion.
 """
 from __future__ import annotations
 
@@ -253,13 +254,20 @@ def uninstall_ulysses() -> None:
 
 
 def _lm_head_eligible(ctx, cls, hidden_states, head_weight, head_bias) -> bool:
-    """what ``ops.lm_head_cross_entropy`` computes: the plain context (``MTPLossContext`` subclasses it with its own
-    ``loss_fn``), no bias, bf16 CUDA hidden states and weight (``fp32_lm_head`` gives fp32), widths multiples of 128"""
-    kw = ctx.loss_kwargs
-    return (type(ctx) is cls and head_bias is None and kw is not None and kw.loss_weight is not None
+    """what the lm_head kernels (``ops.lm_head_cross_entropy``, ``ops.lm_head_logprobs``) compute: the plain context
+    (subclasses such as ``MTPLossContext`` bring their own ``loss_fn``), no bias, bf16 CUDA hidden states and weight
+    (``fp32_lm_head`` gives fp32), widths multiples of 128"""
+    return (type(ctx) is cls and head_bias is None
             and all(type(t) in (torch.Tensor, nn.Parameter) and _on_device(t) and t.dtype == torch.bfloat16
                     for t in (hidden_states, head_weight))
             and head_weight.dim() == 2 and head_weight.shape[0] % 128 == 0 and head_weight.shape[1] % 128 == 0)
+
+
+def _ce_eligible(ctx, cls, hidden_states, head_weight, head_bias) -> bool:
+    """:func:`_lm_head_eligible` for the cross-entropy, which also needs the loss weight ``build_batches`` sets"""
+    kw = ctx.loss_kwargs
+    return (kw is not None and kw.loss_weight is not None
+            and _lm_head_eligible(ctx, cls, hidden_states, head_weight, head_bias))
 
 
 def _lm_head_loss(ctx, hidden_states, head_weight, loss_kwargs, chunk_size):
@@ -285,14 +293,14 @@ def install_lm_head_loss() -> None:
     orig_eager, orig_chunk = vars(cls)["eager_mode"], vars(cls)["chunk_mode"]
 
     def eager_mode(self, hidden_states, head_weight, head_bias, loss_kwargs):
-        if self.loss_cfg.mode == "eager" and _lm_head_eligible(self, cls, hidden_states, head_weight, head_bias):
+        if self.loss_cfg.mode == "eager" and _ce_eligible(self, cls, hidden_states, head_weight, head_bias):
             return _lm_head_loss(self, hidden_states, head_weight, loss_kwargs, None)
         return orig_eager(self, hidden_states, head_weight, head_bias, loss_kwargs)
 
     def chunk_mode(self, hidden_states, head_weight, head_bias, loss_kwargs):
         if (self.loss_cfg.mode == "chunk" and self.loss_cfg.chunk_size is not None
                 and (hidden_states.dim() == 2 or hidden_states.shape[0] == 1)
-                and _lm_head_eligible(self, cls, hidden_states, head_weight, head_bias)):
+                and _ce_eligible(self, cls, hidden_states, head_weight, head_bias)):
             return _lm_head_loss(self, hidden_states, head_weight, loss_kwargs, self.loss_cfg.chunk_size)
         return orig_chunk(self, hidden_states, head_weight, head_bias, loss_kwargs)
 
@@ -307,6 +315,107 @@ def uninstall_lm_head_loss() -> None:
     if _SAVED in vars(cls):
         cls.eager_mode, cls.chunk_mode = vars(cls)[_SAVED]
         delattr(cls, _SAVED)
+
+
+# ======================================================================================================
+# lm_head label log-probabilities (f5): LogProbContext and GRPOLossContext
+# ======================================================================================================
+
+
+def _policy_extra_info(logprobs, old_logprobs, valid, cliprange_low, cliprange_high) -> dict:
+    """The statistics ``GRPOLossContext.loss_fn`` returns beside its loss, from detached log-probabilities.  With
+    d = logp - old and r = exp(clamp(d, -20, 20)), over the valid positions: the largest and smallest r, the sums of
+    |r - 1|, of k1 = -d and of k3 = r - 1 - clamp(d, -20, 20), their number, and, when both clip bounds are set, how many
+    r lie below 1 - low and above 1 + high.  Invalid positions enter the sums as exact zeros, so each sum runs over the
+    same tensor shape as the reference's and keeps its bits."""
+    d = logprobs.detach() - old_logprobs.detach()
+    d_clamped = d.clamp(-20.0, 20.0)
+    r = d_clamped.exp()
+    on = valid.float()
+    r_max = torch.where(valid, r, 0.0).max()
+    info = {
+        "max_ratio": r_max,
+        "reduced_train_policy_ratio_abs_dev_sum": ((r - 1.0).abs() * on).sum(),
+        "reduced_train_policy_kl1_sum": (d.neg() * on).sum(),
+        "reduced_train_policy_kl3_sum": ((r - 1.0 - d_clamped) * on).sum(),
+        "reduced_train_policy_valid_count": on.sum(),
+        "reduced_train_policy_ratio_max": r_max,
+        "reduced_train_policy_ratio_min": torch.where(valid, r, float("inf")).min(),
+    }
+    if cliprange_low is not None and cliprange_high is not None:
+        info["reduced_train_policy_clip_low_count"] = (valid & (r < 1 - cliprange_low)).float().sum()
+        info["reduced_train_policy_clip_high_count"] = (valid & (r > 1 + cliprange_high)).float().sum()
+    return info
+
+
+def install_rl_lm_head() -> None:
+    """Moves the lm_head of the RL trainer's three calls per micro-batch onto :func:`ops.lm_head_logprobs`:
+
+    * ``LogProbContext.loss_fn`` and ``.chunk_mode`` (``xtuner/v1/loss/rl_loss.py``; the actor's and the reference
+      model's log-probabilities) return ``(ops.lm_head_logprobs(...), (None, {}))``;
+    * ``GRPOLossContext.loss_fn`` (``xtuner/v1/rl/loss/grpo_loss.py``) takes the log-probabilities from the op and runs
+      the context's own ``policy_loss_fn`` and, with ``use_kl_loss``, ``kl_penalty`` on them in torch, so every registered
+      loss type and KL type is served; it returns ``(loss, (None, extra_info))`` with the reference's statistics.  Modes
+      "eager" and "chunk" both reach it (chunk mode through ``ChunkLoss``).
+
+    Calls it does not cover go to the original methods: subclasses with their own ``loss_fn`` (``OrealLossContext``),
+    mode ``"liger"``, a head bias, fp32 or non-CUDA tensors, a weight that is not a plain tensor, ``V`` or ``H`` not a
+    multiple of 128.  Opt-in because the served calls return no logits.  Composes with :func:`install_lm_head_loss` in
+    either order.  The RL modules (which import ``ray``) are loaded here only."""
+    lp_cls = importlib.import_module("xtuner.v1.loss.rl_loss").LogProbContext
+    grpo_mod = importlib.import_module("xtuner.v1.rl.loss.grpo_loss")
+    grpo_cls = grpo_mod.GRPOLossContext
+    if _SAVED in vars(grpo_cls):
+        return
+    lp_loss_fn, lp_chunk_mode = vars(lp_cls)["loss_fn"], vars(lp_cls)["chunk_mode"]
+    grpo_loss_fn = vars(grpo_cls)["loss_fn"]
+
+    def logprob_loss_fn(self, hidden_states, head_weight, head_bias, loss_kwargs):
+        if _lm_head_eligible(self, lp_cls, hidden_states, head_weight, head_bias):
+            return ops.lm_head_logprobs(hidden_states, head_weight, loss_kwargs.shifted_labels), (None, {})
+        return lp_loss_fn(self, hidden_states, head_weight, head_bias, loss_kwargs)
+
+    def logprob_chunk_mode(self, hidden_states, head_weight, head_bias, loss_kwargs):
+        if (self.loss_cfg.chunk_size is not None
+                and _lm_head_eligible(self, lp_cls, hidden_states, head_weight, head_bias)):
+            logprobs = ops.lm_head_logprobs(hidden_states, head_weight, loss_kwargs.shifted_labels,
+                                            self.loss_cfg.chunk_size)
+            return logprobs, (None, {})
+        return lp_chunk_mode(self, hidden_states, head_weight, head_bias, loss_kwargs)
+
+    def grpo_loss(self, hidden_states, head_weight, head_bias, loss_kwargs):
+        if not (self.loss_cfg.mode in ("eager", "chunk")
+                and _lm_head_eligible(self, grpo_cls, hidden_states, head_weight, head_bias)):
+            return grpo_loss_fn(self, hidden_states, head_weight, head_bias, loss_kwargs)
+        cfg = self.loss_cfg
+        labels = loss_kwargs.shifted_labels
+        logprobs = ops.lm_head_logprobs(hidden_states, head_weight, labels)
+        loss = self.policy_loss_fn(logprobs, loss_kwargs.old_logprobs, loss_kwargs.advantages,
+                                   loss_kwargs.policy_loss_weight, cfg.policy_loss_cfg)
+        extra_info = _policy_extra_info(logprobs, loss_kwargs.old_logprobs, labels != cfg.ignore_idx,
+                                        cfg.policy_loss_cfg.get("cliprange_low"), cfg.policy_loss_cfg.get("cliprange_high"))
+        if cfg.use_kl_loss:
+            loss = loss + grpo_mod.kl_penalty(logprobs, loss_kwargs.ref_logprobs, loss_kwargs.kl_loss_weight,
+                                              cfg.kl_loss_type)
+        return loss, (None, extra_info)
+
+    logprob_loss_fn.__wrapped__, logprob_chunk_mode.__wrapped__, grpo_loss.__wrapped__ = (lp_loss_fn, lp_chunk_mode,
+                                                                                          grpo_loss_fn)
+    setattr(lp_cls, _SAVED, (lp_loss_fn, lp_chunk_mode))
+    setattr(grpo_cls, _SAVED, (grpo_loss_fn,))
+    lp_cls.loss_fn, lp_cls.chunk_mode = logprob_loss_fn, logprob_chunk_mode
+    grpo_cls.loss_fn = grpo_loss
+
+
+def uninstall_rl_lm_head() -> None:
+    lp_cls = importlib.import_module("xtuner.v1.loss.rl_loss").LogProbContext
+    grpo_cls = importlib.import_module("xtuner.v1.rl.loss.grpo_loss").GRPOLossContext
+    if _SAVED in vars(lp_cls):
+        lp_cls.loss_fn, lp_cls.chunk_mode = vars(lp_cls)[_SAVED]
+        delattr(lp_cls, _SAVED)
+    if _SAVED in vars(grpo_cls):
+        (grpo_cls.loss_fn,) = vars(grpo_cls)[_SAVED]
+        delattr(grpo_cls, _SAVED)
 
 
 # ======================================================================================================
