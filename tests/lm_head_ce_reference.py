@@ -80,3 +80,22 @@ def grad64(z: torch.Tensor, labels: torch.Tensor, loss_weight: torch.Tensor, ign
     p.scatter_add_(1, safe[:, None], -torch.ones_like(p[:, :1]))
     g = p * loss_weight.double()[:, None]
     return torch.where(keep[:, None], g, torch.zeros_like(g))
+
+
+def logp64(z: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
+    """logp_t = log_softmax(z_t)[max(label_t, 0)] in float64 (labels clipped at 0, as gather_logprobs does)"""
+    idx = labels.clamp_min(0)
+    return z.double().gather(1, idx[:, None])[:, 0] - logsumexp64(z)
+
+
+def row_stats64(z: torch.Tensor):
+    """per row (max, log(sum(exp(z - max)))) of bf16 logits, the max exact and the log-sum in float64"""
+    m = z.double().amax(1)
+    return m, torch.log(torch.exp(z.double() - m[:, None]).sum(1))
+
+
+def logprob_grad64(z: torch.Tensor, labels: torch.Tensor, grad_logp: torch.Tensor) -> torch.Tensor:
+    """G = (onehot(max(label, 0)) - softmax(z)) * c in float64 for dL/dlogp = c"""
+    g = -torch.softmax(z.double(), dim=-1)
+    g.scatter_add_(1, labels.clamp_min(0)[:, None], torch.ones_like(g[:, :1]))
+    return g * grad_logp.double()[:, None]

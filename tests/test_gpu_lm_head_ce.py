@@ -57,8 +57,10 @@ def _random(T, H, V, seed, scale=1.0):
     return h, w
 
 
-@pytest.mark.parametrize("V", [512, 384, 1152])  # 256-column tiles; 128-column tiles (V % 256 == 128)
-@pytest.mark.parametrize("T", [1, 100, 128, 1000])
+# 256-column tiles; 128-column tiles (V % 256 == 128); one tile of each width
+@pytest.mark.parametrize("V", [512, 384, 1152, 128, 256])
+# 16-row store boxes: full, and ragged in their first or second 8-row half; 128-row tiles: one short, full, one over
+@pytest.mark.parametrize("T", [1, 100, 128, 1000, 8, 9, 16, 17, 63, 64, 65, 127, 129])
 def test_logits_are_exact_and_stay_inside_the_buffer(T, V):
     H = 256
     h = R.rows_operand([T], H, "exact", seed=T, device=DEV)

@@ -156,6 +156,28 @@ def test_all_ignored_gives_zero_loss_and_zero_gradients(gold, emu, mode):
     assert float(loss) == 0.0 and dh.count_nonzero() == 0 and dw.count_nonzero() == 0
 
 
+@pytest.mark.parametrize("grad", [True, False])
+@pytest.mark.parametrize("chunk", [None, 128])
+def test_zero_rows_make_no_entry_call_and_give_the_references_result(gold, emu, chunk, grad):
+    """An empty tensor has no address, which the entry's null check rejects: zero rows must not reach it."""
+    from xtuner_b200 import ops
+
+    H = gold["hidden"].shape[1]
+    h0 = torch.empty((0, H), dtype=torch.bfloat16)
+    lab0, lw0 = torch.empty((0,), dtype=torch.int64), torch.empty((0,))
+    want = lm_head_ce(h0, gold["weight"], lab0, lw0, gold["ignore_index"], chunk)
+    h = h0.clone().requires_grad_(grad)
+    w = gold["weight"].clone().requires_grad_(grad)
+    loss = ops.lm_head_cross_entropy(h, w, lab0, lw0, gold["ignore_index"], chunk)
+    assert emu.calls == []
+    assert loss.dtype == torch.float32 and loss.shape == () and torch.equal(loss.detach(), want[0])
+    if grad:
+        loss.backward()
+        assert h.grad.shape == (0, H) and torch.equal(h.grad, want[1]) and torch.equal(w.grad, want[2])
+        assert w.grad.count_nonzero() == 0
+    assert emu.calls == []
+
+
 def test_shape_errors_are_raised_on_the_host(gold, emu):
     from xtuner_b200 import _capi, ops
 

@@ -469,12 +469,16 @@ class _LMHeadCrossEntropy(torch.autograd.Function):
     def forward(ctx, h: Tensor, w: Tensor, labels: Tensor, loss_weight: Tensor, ignore_index: int,
                 chunk_size: Optional[int], need_grad: bool):
         T = h.shape[0]
-        step = max(T, 1) if chunk_size is None else chunk_size
+        if T == 0:  # an empty tensor has no address, which the entry rejects; the reference gives 0, empty dh, zero dW
+            if need_grad:
+                ctx.save_for_backward(torch.empty_like(h), torch.zeros_like(w))
+            return torch.zeros((), dtype=torch.float32, device=h.device)
+        step = T if chunk_size is None else chunk_size
         z = torch.empty((min(step, T), w.shape[0]), dtype=torch.bfloat16, device=h.device)  # z, then G, of one chunk
         row_ce = torch.empty((T,), dtype=torch.float32, device=h.device)
         dh = torch.empty_like(h) if need_grad else None
         loss = dw = dw_chunk = None
-        for s in range(0, max(T, 1), step):
+        for s in range(0, T, step):
             n = min(step, T - s)
             loss_c = torch.empty((), dtype=torch.float32, device=h.device)
             dw_c = None
