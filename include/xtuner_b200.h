@@ -304,6 +304,12 @@ int xtb_swiglu(const void* h_bf16, void* out_bf16, int64_t M, int I, xtb_stream_
  * I / 8 <= 23170 (the row split's 32-bit reciprocal). */
 int xtb_swiglu_bwd(const void* grad_out_bf16, const void* h_bf16, void* grad_h_bf16, int64_t M, int I,
                    xtb_stream_t stream);
+/* xtb_swiglu_bwd that also writes the forward's output act_out[M, I] = xtb_swiglu(h) (the same bits as xtb_swiglu and
+ * the xtb_group_gemm_nt_swiglu epilogue) in the same pass: the fused MoE nodes' selective recompute, which drops the
+ * SwiGLU output in the forward (ops/act_fn.py:7-9; MoEBlock.forward, moe_decoder_layer.py:196-200).  Same shape and
+ * alignment rules as xtb_swiglu_bwd. */
+int xtb_swiglu_bwd_act(const void* grad_out_bf16, const void* h_bf16, void* grad_h_bf16, void* act_out_bf16, int64_t M,
+                       int I, xtb_stream_t stream);
 
 /* ==== the step either side of the path (SURVEY.md §8f-3) =================================================
  * post_attention_layernorm (module/decoder_layer/moe_decoder_layer.py:664-679; F.rms_norm via

@@ -154,6 +154,7 @@ SIGNATURES = {
     ),
     "xtb_swiglu": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "xtb_swiglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "xtb_swiglu_bwd_act": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
 }
 
 

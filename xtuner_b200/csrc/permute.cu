@@ -350,12 +350,16 @@ __global__ void __launch_bounds__(256) swiglu_kernel(const uint4* __restrict__ h
 }
 
 // One element pair of the SwiGLU backward with the reference's rounding points (ops/act_fn.py:7-9 under autograd).
-__device__ __forceinline__ void swiglu_bwd_vec(const uint4& g, const uint4& u, const uint4& go, uint4& o_g, uint4& o_u) {
+// kAct also gives the forward's output a = bf16(s * x2) from the s it recomputes: the product swiglu_kernel and the
+// nt_swiglu GEMM epilogue round, so the bits are theirs.
+template <bool kAct>
+__device__ __forceinline__ void swiglu_bwd_vec(const uint4& g, const uint4& u, const uint4& go, uint4& o_g, uint4& o_u,
+                                               uint4& o_a) {
   const uint32_t gw[4] = {g.x, g.y, g.z, g.w}, uw[4] = {u.x, u.y, u.z, u.w}, dw[4] = {go.x, go.y, go.z, go.w};
-  uint32_t o1[4], o2[4];
+  uint32_t o1[4], o2[4], oa[4];
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    float x1[2], x2[2], d[2], r1[2], r2[2];
+    float x1[2], x2[2], d[2], r1[2], r2[2], ra[2];
     unpack_bf16x2(gw[q], x1[0], x1[1]);
     unpack_bf16x2(uw[q], x2[0], x2[1]);
     unpack_bf16x2(dw[q], d[0], d[1]);
@@ -366,21 +370,27 @@ __device__ __forceinline__ void swiglu_bwd_vec(const uint4& g, const uint4& u, c
       r2[z] = d[z] * s;                           // grad wrt x2  (rounded at pack)
       const float ds = round_bf16(d[z] * x2[z]);  // grad wrt silu output, a bf16 tensor in the reference
       r1[z] = ds * sig * (1.f + x1[z] * (1.f - sig));
+      if (kAct) ra[z] = s * x2[z];                // the forward's output (rounded at pack)
     }
     o1[q] = pack_bf16x2(r1[0], r1[1]);
     o2[q] = pack_bf16x2(r2[0], r2[1]);
+    if (kAct) oa[q] = pack_bf16x2(ra[0], ra[1]);
   }
   o_g = make_uint4(o1[0], o1[1], o1[2], o1[3]);
   o_u = make_uint4(o2[0], o2[1], o2[2], o2[3]);
+  if (kAct) o_a = make_uint4(oa[0], oa[1], oa[2], oa[3]);
 }
 
 // A 64-bit divide per thread to find its row, with one 16-byte vector per thread, is instruction-bound.  A block owns
 // kSwRows consecutive rows, the row of a vector comes from a
 // 32-bit multiply-high with a host-made reciprocal, and every thread keeps two vectors' loads in flight.
+// kAct: also write the forward's output to act ([M, I], the rows of grad_out).
 constexpr int kSwRows = 8;
+template <bool kAct>
 __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const uint4* __restrict__ grad_out,
                                                          const uint4* __restrict__ h, uint4* __restrict__ grad_h,
-                                                         int64_t M, int I8, uint32_t inv_I8 /* ceil(2^32 / I8) */) {
+                                                         int64_t M, int I8, uint32_t inv_I8 /* ceil(2^32 / I8) */,
+                                                         uint4* __restrict__ act) {
   pdl_sync();
   const int64_t m0 = (int64_t)blockIdx.x * kSwRows;
   const int rows = (int)min((int64_t)kSwRows, M - m0);
@@ -405,10 +415,11 @@ __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const uint4* __restrict
 #pragma unroll
     for (int k = 0; k < 2; ++k) {
       if (i[k] < n) {
-        uint4 og, ou;
-        swiglu_bwd_vec(g[k], u[k], go[k], og, ou);
+        uint4 og, ou, oa;
+        swiglu_bwd_vec<kAct>(g[k], u[k], go[k], og, ou, oa);
         st_stream_16(ob + (size_t)r[k] * (2 * I8) + j[k], og);
         st_stream_16(ob + (size_t)r[k] * (2 * I8) + I8 + j[k], ou);
+        if (kAct) st_stream_16(act + m0 * I8 + i[k], oa);
       }
     }
   }
@@ -563,6 +574,30 @@ extern "C" int xtb_swiglu(const void* h_bf16, void* out_bf16, int64_t M, int I, 
   return XTB_OK;
 }
 
+// xtb_swiglu_bwd (act_out == NULL) and xtb_swiglu_bwd_act; `entry` names the one that was called in the refusal messages
+static int swiglu_bwd_impl(const char* entry, const void* grad_out_bf16, const void* h_bf16, void* grad_h_bf16,
+                           void* act_out_bf16, int64_t M, int I, xtb_stream_t stream) {
+  const int I8 = I / 8;
+  // floor(i / I8) == umulhi(i, ceil(2^32 / I8)) as long as i * I8 < 2^32; i < kSwRows * I8 inside a block
+  XTB_CHECK_ARG((int64_t)kSwRows * I8 * I8 < (1ll << 32), "%s: I=%d too wide", entry, I);
+  XTB_ENSURE_CTX(h_bf16);
+  if (M == 0) return XTB_OK;
+  const uint32_t inv_I8 = (uint32_t)(((1ull << 32) + I8 - 1) / I8);
+  const dim3 grid((unsigned)((M + kSwRows - 1) / kSwRows));
+  const auto* go = static_cast<const uint4*>(grad_out_bf16);
+  const auto* h = static_cast<const uint4*>(h_bf16);
+  auto* gh = static_cast<uint4*>(grad_h_bf16);
+  if (act_out_bf16) {
+    XTB_CUDA(launch_pdl(swiglu_bwd_kernel<true>, grid, dim3(256), 0, as_stream(stream), go, h, gh, M, I8, inv_I8,
+                        static_cast<uint4*>(act_out_bf16)));
+  } else {
+    XTB_CUDA(launch_pdl(swiglu_bwd_kernel<false>, grid, dim3(256), 0, as_stream(stream), go, h, gh, M, I8, inv_I8,
+                        static_cast<uint4*>(nullptr)));
+  }
+  XTB_LAUNCH_OK();
+  return XTB_OK;
+}
+
 extern "C" int xtb_swiglu_bwd(const void* grad_out_bf16, const void* h_bf16, void* grad_h_bf16, int64_t M, int I,
                               xtb_stream_t stream) {
   XTB_CHECK_ARG(grad_out_bf16 && h_bf16 && grad_h_bf16, "xtb_swiglu_bwd: null pointer");
@@ -570,17 +605,15 @@ extern "C" int xtb_swiglu_bwd(const void* grad_out_bf16, const void* h_bf16, voi
   XTB_CHECK_ARG((reinterpret_cast<uintptr_t>(grad_out_bf16) | reinterpret_cast<uintptr_t>(h_bf16) |
                  reinterpret_cast<uintptr_t>(grad_h_bf16)) % 16 == 0,
                 "xtb_swiglu_bwd: pointers must be 16-byte aligned");
-  const int64_t n = M * (I / 8);
-  const int I8 = I / 8;
-  // floor(i / I8) == umulhi(i, ceil(2^32 / I8)) as long as i * I8 < 2^32; i < kSwRows * I8 inside a block
-  XTB_CHECK_ARG((int64_t)kSwRows * I8 * I8 < (1ll << 32), "xtb_swiglu_bwd: I=%d too wide", I);
-  XTB_ENSURE_CTX(h_bf16);
-  if (M == 0) return XTB_OK;
-  const uint32_t inv_I8 = (uint32_t)(((1ull << 32) + I8 - 1) / I8);
-  (void)n;
-  XTB_CUDA(launch_pdl(swiglu_bwd_kernel, dim3((unsigned)((M + kSwRows - 1) / kSwRows)), dim3(256), 0, as_stream(stream), 
-      static_cast<const uint4*>(grad_out_bf16), static_cast<const uint4*>(h_bf16), static_cast<uint4*>(grad_h_bf16),
-      M, I8, inv_I8));
-  XTB_LAUNCH_OK();
-  return XTB_OK;
+  return swiglu_bwd_impl("xtb_swiglu_bwd", grad_out_bf16, h_bf16, grad_h_bf16, nullptr, M, I, stream);
+}
+
+extern "C" int xtb_swiglu_bwd_act(const void* grad_out_bf16, const void* h_bf16, void* grad_h_bf16, void* act_out_bf16,
+                                  int64_t M, int I, xtb_stream_t stream) {
+  XTB_CHECK_ARG(grad_out_bf16 && h_bf16 && grad_h_bf16 && act_out_bf16, "xtb_swiglu_bwd_act: null pointer");
+  XTB_CHECK_ARG(M >= 0 && I > 0 && I % 8 == 0, "xtb_swiglu_bwd_act: bad shape");
+  XTB_CHECK_ARG((reinterpret_cast<uintptr_t>(grad_out_bf16) | reinterpret_cast<uintptr_t>(h_bf16) |
+                 reinterpret_cast<uintptr_t>(grad_h_bf16) | reinterpret_cast<uintptr_t>(act_out_bf16)) % 16 == 0,
+                "xtb_swiglu_bwd_act: pointers must be 16-byte aligned");
+  return swiglu_bwd_impl("xtb_swiglu_bwd_act", grad_out_bf16, h_bf16, grad_h_bf16, act_out_bf16, M, I, stream);
 }

@@ -14,7 +14,9 @@ With ``fused=True`` the MoE half of every eligible layer (``post_attention_layer
 experts -> combine -> ``* hidden_factor + residual``, ``moe_decoder_layer.py:668-705,411-488``) additionally runs as ONE
 autograd node (:func:`xtuner_b200.fused.fused_moe_block`), the form ``bench.py`` measures, rollout-routed experts (RL
 routing replay) included; the per-op classes above stay installed for the path the fused node does not cover
-(micro-batched forward).
+(micro-batched forward).  ``recompute="act"`` or ``"experts"`` (with ``fused=True`` only) has every fused node rebuild
+some of its expert intermediates in the backward instead of keeping them (:data:`xtuner_b200.fused.RECOMPUTE`): less
+activation memory for the same results, without checkpointing the whole decoder layer.
 
 Everything else of the model (attention, norms, lm_head, FSDP wrapping, checkpoint keys) is untouched;
 ``install_lm_head_loss()`` separately moves the lm_head cross-entropy onto this package's kernels,
@@ -113,30 +115,38 @@ def _fused_layer_forward(self, hidden_states, seq_ctx, position_embeddings):
     router = self.gate.router
     # RL routing replay: this layer's slice of the [S, L, K] ids, moved to the device if offloaded, exactly as the
     # reference does (moe_decoder_layer.py:669-677)
-    replay = {}  # the keyword only when there are ids: the routing call keeps fused_moe_block's own defaults
+    opts = {}  # keywords only when set: the call keeps fused_moe_block's own defaults
     ids = getattr(seq_ctx, "rollout_routed_experts", None)
     if ids is not None and self.layer_idx < ids.shape[1]:
         ids = ids[:, self.layer_idx, :]
         if seq_ctx.offload_rollout_routed_experts and ids.device != hidden_states.device:
             ids = ids.contiguous().to(hidden_states.device)
-        replay["rollout_routed_experts"] = ids
+        opts["rollout_routed_experts"] = ids
+    recompute = vars(self).get(_SAVED, {}).get("recompute")
+    if recompute is not None:
+        opts["recompute"] = recompute
     out, rr = _fused.fused_moe_block(
         hidden_states, _local(self.post_attention_layernorm.weight), self.post_attention_layernorm.variance_epsilon,
         _local(self.gate.weight), _local(self.experts.fused_w1w3.weight), _local(self.experts.fused_w2.weight),
         top_k=router.top_k, norm_topk_prob=router.norm_topk_prob, router_scaling_factor=router.router_scaling_factor,
-        hidden_factor=self.hidden_factor, scoring_func=router.scoring_func, **replay,
+        hidden_factor=self.hidden_factor, scoring_func=router.scoring_func, **opts,
     )
     return out, rr["logits"], rr["router_weights"], rr["topk_ids"]
 
 
-def convert_model(model: nn.Module, *, swiglu: bool = True, fused: bool = False, ep: "bool | str" = False) -> int:
+def convert_model(model: nn.Module, *, swiglu: bool = True, fused: bool = False, ep: "bool | str" = False,
+                  recompute: "str | None" = None) -> int:
     """Returns the number of MoE decoder layers converted.  ``ep`` also converts ``TorchAll2AllDispatcher`` layers (expert
     parallel): ``True`` / ``"nccl"`` -> :class:`All2AllDispatcher` (the reference's six phases, NCCL all-to-all, our
     permute/unpermute kernels); ``"peer"`` -> :class:`PeerAll2AllDispatcher` (device-side split sizes, peer-memory pull
     kernels, no host read; needs symmetric memory over the EP group).  Both are covered by ``tests/test_gpu_comm.py`` with
-    ``XTB_TEST_EP=1`` on >= 2 GPUs."""
+    ``XTB_TEST_EP=1`` on >= 2 GPUs.  ``recompute`` (``"act"`` or ``"experts"``, needs ``fused=True``): what the fused nodes
+    rebuild in the backward, as in :func:`xtuner_b200.fused.fused_moe_block`."""
     if ep not in (False, True, "nccl", "peer"):
         raise ValueError(f"convert_model: ep must be False, True, 'nccl' or 'peer' (got {ep!r})")
+    _fused._check_recompute("convert_model", recompute)
+    if recompute is not None and not fused:
+        raise ValueError(f"convert_model: recompute={recompute!r} applies to the fused nodes: it needs fused=True")
     n = 0
     for layer in model.modules():
         # the layer itself, not a wrapper that forwards attribute reads to it (torch's CheckpointWrapper under the
@@ -174,6 +184,7 @@ def convert_model(model: nn.Module, *, swiglu: bool = True, fused: bool = False,
             layer.experts.moe_act = ops.swiglu
         if fused and kind == "NaiveDispatcher" and _fused_eligible(layer):
             saved["fused_forward"] = True
+            saved["recompute"] = recompute
             layer._forward = types.MethodType(_fused_layer_forward, layer)  # instance attribute shadows the class method
         setattr(layer, _SAVED, saved)
         n += 1
