@@ -18,6 +18,7 @@ Copies are compared bit for bit; a NaN is compared by position only (the CUDA ca
   barrier with world > 1 waits for peers that do not exist on one device, so this file never launches one.
 * One a2a and one EP case whose addresses pass 2^31 bytes.
 """
+import contextlib
 import ctypes
 
 import numpy as np
@@ -25,43 +26,23 @@ import pytest
 import torch
 
 from tests import exchange_reference as R
+from tests.gpu_harness import XTB_ERR_INVALID, Worst, sm_count
+from xtuner_b200._capi import check, current_stream, ensure_init, ptr
 
 pytestmark = pytest.mark.gpu
 
-XTB_ERR_INVALID = 1
-WORST = {}  # quantity -> largest |err| / bound in random mode (printed at the end of the module)
+WORST = Worst("exchange_single_device")  # in random mode
 PEAK = {}
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _report():
+@contextlib.contextmanager
+def _peaks():
     yield
-    for k, v in sorted(WORST.items()):
-        print(f"exchange_single_device: {k}: {v:.4g}")
     for k, v in sorted(PEAK.items()):
         print(f"exchange_single_device: peak memory {k}: {v / 2**30:.2f} GiB")
 
 
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi.ensure_init()
-
-
-def _st():
-    from xtuner_b200._capi import current_stream
-
-    return current_stream()
-
-
-def _ok(rc, what):
-    from xtuner_b200._capi import check
-
-    check(rc, what)
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
+_report = WORST.fixture(_peaks)
 
 
 def _t(x):
@@ -126,7 +107,8 @@ def _run_a2a(inputs, s, g, what):
     for r in range(W):
         plan = a2a_plan(shape, s, g, W, r, es)
         o = R.guarded(nbytes)
-        _ok(_lib().xtb_a2a_pull(world.table.data_ptr(), o.ptr(0), r, W, *_a2a_args(plan), _st()), "xtb_a2a_pull")
+        check(ensure_init().xtb_a2a_pull(world.table.data_ptr(), o.ptr(0), r, W, *_a2a_args(plan), current_stream()),
+              "xtb_a2a_pull")
         outs.append((o, plan))
     torch.cuda.synchronize()
     got = []
@@ -155,7 +137,7 @@ def test_a2a_pull_matches_reference_and_round_trips(shape, dtype, s, g, W):
 def test_a2a_pull_grid_stride_step(W, delta):
     """16-byte rows, so the total is the row count: one grid-stride step of a source's blocks is per_src * 256 * 8
     vectors, per_src capped at 2 * SMs / W.  Totals just below, at and just above one full step."""
-    cap = max(1, 2 * _sms() // W)
+    cap = max(1, 2 * sm_count() // W)
     total = cap * 256 * 8 + delta
     inputs = [R.labels(W * total * 16, r).view(torch.int16).view(W * total, 8) for r in range(W)]
     _run_a2a(inputs, 0, 1, f"a2a total={total}")
@@ -164,7 +146,7 @@ def test_a2a_pull_grid_stride_step(W, delta):
 def test_a2a_pull_refusals():
     from xtuner_b200.comm import a2a_plan
 
-    lib, W = _lib(), 2
+    lib, W = ensure_init(), 2
     shape = (2 * W, 64)
     world = R.SimWorld(W, 2 * W * 64 * 2)
     o = R.guarded(2 * W * 64 * 2)
@@ -175,9 +157,10 @@ def test_a2a_pull_refusals():
     for k, name in enumerate(names):
         bad = list(args)
         bad[3 + k] += 8
-        rc = lib.xtb_a2a_pull(world.table.data_ptr(), o.ptr(0), 1, W, *bad, _st())
+        rc = lib.xtb_a2a_pull(world.table.data_ptr(), o.ptr(0), 1, W, *bad, current_stream())
         assert rc == XTB_ERR_INVALID, f"{name} not a multiple of 16 was accepted"
-    assert lib.xtb_a2a_pull(world.table.data_ptr(), o.ptr(0), 1, W, *args[:3], 0, *args[4:], _st()) == XTB_ERR_INVALID
+    assert lib.xtb_a2a_pull(world.table.data_ptr(), o.ptr(0), 1, W, *args[:3], 0, *args[4:],
+                            current_stream()) == XTB_ERR_INVALID
     assert lib.xtb_launch_count() == n0
     torch.cuda.synchronize()
     assert bool((o.arena == R.FILL32).all())
@@ -187,20 +170,21 @@ def test_a2a_pull_refusals():
 
 
 def _ag_n(kind):
-    return {"8": 8, "tail": 8 * (3 * 2048 + 5), "waves": 8 * (4 * 2 * _sms() * 256 + 3)}[kind]
+    return {"8": 8, "tail": 8 * (3 * 2048 + 5), "waves": 8 * (4 * 2 * sm_count() * 256 + 3)}[kind]
 
 
 @pytest.mark.parametrize("W", [1, 2, 3, 8])
 @pytest.mark.parametrize("f32", [True, False], ids=["f32", "bf16"])
 @pytest.mark.parametrize("kind", ["8", "tail", "waves"])
 def test_allgather_push(W, f32, kind):
-    lib, n = _lib(), _ag_n(kind)
+    lib, n = ensure_init(), _ag_n(kind)
     shards = [R.f32_specials(n, seed=r) for r in range(W)]
     if not f32:
         shards = [x.to(torch.bfloat16) for x in shards]
     outs = R.SimWorld(W, W * n * 2)
     for r in range(W):
-        _ok(lib.xtb_allgather_push(shards[r].data_ptr(), outs.table.data_ptr(), r, W, n, int(f32), _st()), "xtb_allgather_push")
+        check(lib.xtb_allgather_push(shards[r].data_ptr(), outs.table.data_ptr(), r, W, n, int(f32), current_stream()),
+              "xtb_allgather_push")
     torch.cuda.synchronize()
     want = R.allgather(shards)
     for d in range(W):
@@ -219,7 +203,7 @@ def _scales(W):
 @pytest.mark.parametrize("out_f32", [True, False], ids=["f32out", "bf16out"])
 @pytest.mark.parametrize("mode", ["exact", "random"])
 def test_reduce_scatter_pull(W, out_f32, mode):
-    lib, n = _lib(), 8 * 4099
+    lib, n = ensure_init(), 8 * 4099
     x = R.rank_values(W, W * n, mode, seed=100 * W + out_f32)
     world = R.SimWorld(W, W * n * 2)
     for r in range(W):
@@ -229,8 +213,8 @@ def test_reduce_scatter_pull(W, out_f32, mode):
         outs = []
         for me in range(W):
             o = R.guarded(n * es)
-            _ok(lib.xtb_reduce_scatter_pull(world.table.data_ptr(), o.ptr(0), me, W, n, scale, int(out_f32), _st()),
-                "xtb_reduce_scatter_pull")
+            check(lib.xtb_reduce_scatter_pull(world.table.data_ptr(), o.ptr(0), me, W, n, scale, int(out_f32),
+                                              current_stream()), "xtb_reduce_scatter_pull")
             outs.append(o)
         torch.cuda.synchronize()
         for me, o in enumerate(outs):
@@ -243,8 +227,7 @@ def test_reduce_scatter_pull(W, out_f32, mode):
                 exact = ref64.float() if out_f32 else R.bf16_rne(ref64.float())
                 R.assert_bits_equal(got, exact, what + " (exact sum)")
             else:
-                WORST[f"reduce_scatter {'f32' if out_f32 else 'bf16'} out"] = max(
-                    WORST.get(f"reduce_scatter {'f32' if out_f32 else 'bf16'} out", 0.0), ratio)
+                WORST.note(f"reduce_scatter {'f32' if out_f32 else 'bf16'} out", ratio)
             assert o.guards_intact(), what + ": wrote outside its output"
     assert world.guards_intact()
 
@@ -252,7 +235,7 @@ def test_reduce_scatter_pull(W, out_f32, mode):
 @pytest.mark.parametrize("W", list(range(1, 17)))
 @pytest.mark.parametrize("mode", ["exact", "random"])
 def test_allreduce_pull_f32(W, mode):
-    lib, n = _lib(), 4 * 8195
+    lib, n = ensure_init(), 4 * 8195
     x = R.rank_values(W, n, mode, seed=7 * W, dtype=torch.float32)
     world = R.SimWorld(W, n * 4)
     for r in range(W):
@@ -261,7 +244,8 @@ def test_allreduce_pull_f32(W, mode):
     outs = []
     for me in range(W):
         o = R.guarded(n * 4)
-        _ok(lib.xtb_allreduce_pull_f32(world.table.data_ptr(), o.ptr(0), me, W, n, scale, _st()), "xtb_allreduce_pull_f32")
+        check(lib.xtb_allreduce_pull_f32(world.table.data_ptr(), o.ptr(0), me, W, n, scale, current_stream()),
+              "xtb_allreduce_pull_f32")
         outs.append(o)
     torch.cuda.synchronize()
     want = R.allreduce(x, scale)
@@ -274,7 +258,7 @@ def test_allreduce_pull_f32(W, mode):
         if mode == "exact":
             R.assert_bits_equal(got, ref64.float(), "all-reduce exact sum")
         else:
-            WORST["allreduce f32"] = max(WORST.get("allreduce f32", 0.0), ratio)
+            WORST.note("allreduce f32", ratio)
         assert o.guards_intact()
 
 
@@ -286,7 +270,7 @@ def test_ep_write_header(E):
     tpe = torch.randint(0, 2**31 - 1, (E,), dtype=torch.int64, device="cuda")
     tpe[0] = 2**31 - 1
     o = R.guarded(4 * E)
-    _ok(_lib().xtb_ep_write_header(tpe.data_ptr(), o.ptr(0), E, _st()), "xtb_ep_write_header")
+    check(ensure_init().xtb_ep_write_header(tpe.data_ptr(), o.ptr(0), E, current_stream()), "xtb_ep_write_header")
     torch.cuda.synchronize()
     assert torch.equal(o.buf(0, torch.int32), tpe.to(torch.int32))
     assert o.guards_intact()
@@ -308,7 +292,8 @@ class _EP:
         self.te_all = [R.ep_to_experts(cnt, d) for d in range(self.W)]
         for s in range(self.W):
             tpe = _t(cnt[s].astype(np.int64))
-            _ok(_lib().xtb_ep_write_header(tpe.data_ptr(), self.src.ptr(s), self.E, _st()), "xtb_ep_write_header")
+            check(ensure_init().xtb_ep_write_header(tpe.data_ptr(), self.src.ptr(s), self.E, current_stream()),
+                  "xtb_ep_write_header")
             torch.cuda.synchronize()
             if self.M[s]:
                 self.src.bytes(s)[self.hdr : self.hdr + self.M[s] * row_bytes].copy_(self.rows[s].view(torch.uint8).view(-1))
@@ -321,20 +306,20 @@ class _EP:
 
     def to_experts(self, own, d, cap, first=True, status_init=(-1, 0)):
         """pull for owner d into own's buffer d; returns (cnt_all_out, tpe_local, status) of the first-use path."""
-        lib = _lib()
+        lib = ensure_init()
         cnt_out = torch.full((self.W * self.E,), -7, dtype=torch.int32, device="cuda") if first else None
         tpe = torch.full((self.El,), -7, dtype=torch.int64, device="cuda") if first else None
         status = torch.tensor(status_init, dtype=torch.int32, device="cuda") if first else None
-        p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        _ok(lib.xtb_ep_pull_to_experts(self.src.table.data_ptr(), None if first else self.cnt_dev.data_ptr(), p(cnt_out),
-                                       own.ptr(d, self.hdr), p(tpe), p(status), d, self.W, self.E, self.rb, self.hdr, cap,
-                                       _st()), "xtb_ep_pull_to_experts")
+        check(lib.xtb_ep_pull_to_experts(self.src.table.data_ptr(), None if first else self.cnt_dev.data_ptr(),
+                                         ptr(cnt_out), own.ptr(d, self.hdr), ptr(tpe), ptr(status), d, self.W, self.E,
+                                         self.rb, self.hdr, cap, current_stream()), "xtb_ep_pull_to_experts")
         return cnt_out, tpe, status
 
     def to_sources(self, own, s, cap, m_rows):
         out = R.guarded(max(self.M[s], 1) * self.rb)
-        _ok(_lib().xtb_ep_pull_to_sources(own.table.data_ptr(), self.cnt_dev.data_ptr(), out.ptr(0), s, self.W, self.E, self.rb,
-                                          self.hdr, cap, m_rows, _st()), "xtb_ep_pull_to_sources")
+        check(ensure_init().xtb_ep_pull_to_sources(own.table.data_ptr(), self.cnt_dev.data_ptr(), out.ptr(0), s, self.W,
+                                                   self.E, self.rb, self.hdr, cap, m_rows, current_stream()),
+              "xtb_ep_pull_to_sources")
         return out
 
     def check_first_use(self, d, cnt_out, tpe, status, cap):
@@ -388,7 +373,7 @@ def test_ep_pulls_match_reference(W, E, load):
 def test_ep_pull_more_rows_than_warps():
     """one owner receives more rows than the 2 * SMs * 8 warps of the grid (and rows of 48 bytes: no 8-vector batch)"""
     W, E = 2, 8
-    n_warps = 2 * _sms() * 8
+    n_warps = 2 * sm_count() * 8
     cnt = np.zeros((W, E), dtype=np.int64)
     cnt[:, 4:] = (n_warps + 37) // 4
     ep = _EP(cnt, 48)
@@ -433,17 +418,18 @@ def test_ep_capacity_and_m_rows():
 
 
 def test_ep_refusals():
-    lib = _lib()
+    lib = ensure_init()
     cnt = np.ones((2, 8), dtype=np.int64)
     ep = _EP(cnt, 16)
     own = ep.owners(16)
     table, cd, dst = ep.src.table.data_ptr(), ep.cnt_dev.data_ptr(), own.ptr(0, ep.hdr)
 
     def te(world=2, E=8, rb=16, hdr=256, cin=cd, cout=None, rank=0):
-        return lib.xtb_ep_pull_to_experts(table, cin, cout, dst, None, None, rank, world, E, rb, hdr, 16, _st())
+        return lib.xtb_ep_pull_to_experts(table, cin, cout, dst, None, None, rank, world, E, rb, hdr, 16,
+                                          current_stream())
 
     def ts(world=2, E=8, rb=16, hdr=256, rank=0):
-        return lib.xtb_ep_pull_to_sources(table, cd, dst, rank, world, E, rb, hdr, 16, 8, _st())
+        return lib.xtb_ep_pull_to_sources(table, cd, dst, rank, world, E, rb, hdr, 16, 8, current_stream())
 
     n0 = lib.xtb_launch_count()
     for f in (te, ts):
@@ -491,7 +477,7 @@ def test_ep_end_to_end_matches_ep1():
     g_x1, g_w13_1, g_w2_1 = torch.autograd.grad(ref, (x1, w13_1, w2_1), torch.cat(gos))
 
     # ep = W on one device
-    lib, rb = _lib(), 2 * H
+    lib, rb = ensure_init(), 2 * H
     hdr = R.ep_hdr_bytes(E)
     x_s = [x.clone().requires_grad_(True) for x in xs]
     perm = [ops.permute(x_s[s], ids[s], n_experts=E, return_extra=True) for s in range(W)]
@@ -505,7 +491,8 @@ def test_ep_end_to_end_matches_ep1():
         wld = R.SimWorld(W, hdr + max(max(len(t) for t in tensors), 1) * rb)
         for r, t in enumerate(tensors):
             if header_tpe is not None:
-                _ok(lib.xtb_ep_write_header(header_tpe[r].data_ptr(), wld.ptr(r), E, _st()), "xtb_ep_write_header")
+                check(lib.xtb_ep_write_header(header_tpe[r].data_ptr(), wld.ptr(r), E, current_stream()),
+                      "xtb_ep_write_header")
             if len(t):
                 wld.bytes(r)[hdr : hdr + len(t) * rb].copy_(t.detach().contiguous().view(torch.uint8).view(-1))
         return wld
@@ -515,9 +502,9 @@ def test_ep_end_to_end_matches_ep1():
         tpes, cnt_out = [], torch.empty(W * E, dtype=torch.int32, device="cuda")
         for d in range(W):
             tl = torch.empty(El, dtype=torch.int64, device="cuda")
-            _ok(lib.xtb_ep_pull_to_experts(src.table.data_ptr(), None if first else cnt_dev.data_ptr(),
-                                           cnt_out.data_ptr() if first else None, own.ptr(d, hdr), tl.data_ptr(), None,
-                                           d, W, E, rb, hdr, cap, _st()), "xtb_ep_pull_to_experts")
+            check(lib.xtb_ep_pull_to_experts(src.table.data_ptr(), None if first else cnt_dev.data_ptr(),
+                                             cnt_out.data_ptr() if first else None, own.ptr(d, hdr), tl.data_ptr(),
+                                             None, d, W, E, rb, hdr, cap, current_stream()), "xtb_ep_pull_to_experts")
             tpes.append(tl)
         rows = [own.bytes(d)[hdr : hdr + n_own[d] * rb].view(torch.bfloat16).view(-1, H) for d in range(W)]
         return rows, tpes
@@ -526,8 +513,8 @@ def test_ep_end_to_end_matches_ep1():
         outs = []
         for s in range(W):
             o = torch.empty(M[s], H, dtype=torch.bfloat16, device="cuda")
-            _ok(lib.xtb_ep_pull_to_sources(own.table.data_ptr(), cnt_dev.data_ptr(), o.data_ptr(), s, W, E, rb, hdr, cap, M[s],
-                                           _st()), "xtb_ep_pull_to_sources")
+            check(lib.xtb_ep_pull_to_sources(own.table.data_ptr(), cnt_dev.data_ptr(), o.data_ptr(), s, W, E, rb, hdr,
+                                             cap, M[s], current_stream()), "xtb_ep_pull_to_sources")
             outs.append(o)
         return outs
 
@@ -560,7 +547,7 @@ def _batch(dsts, srcs, nbytes):
 
 
 def test_peer_memcpy_batch():
-    lib = _lib()
+    lib = ensure_init()
     sizes = [1, 3, 17, 4097, 0, 65535]
     src = R.labels(1 << 20, 3)
     dst = R.guarded(1 << 20)
@@ -568,7 +555,7 @@ def test_peer_memcpy_batch():
     d_ptrs = [dst.ptr(0, o) for o in offs] + [src.data_ptr()]
     s_ptrs = [src.data_ptr() + o + 5 for o in offs] + [src.data_ptr()]  # the last entry has dst == src: skipped
     nb = sizes + [64]
-    _ok(lib.xtb_peer_memcpy_batch(*_batch(d_ptrs, s_ptrs, nb), len(nb), _st()), "xtb_peer_memcpy_batch")
+    check(lib.xtb_peer_memcpy_batch(*_batch(d_ptrs, s_ptrs, nb), len(nb), current_stream()), "xtb_peer_memcpy_batch")
     torch.cuda.synchronize()
     want = torch.full((1 << 20,), 0, dtype=torch.uint8, device="cuda")
     want.view(torch.int32).fill_(R.FILL32)
@@ -578,26 +565,27 @@ def test_peer_memcpy_batch():
     assert dst.guards_intact()
     assert torch.equal(src, R.labels(1 << 20, 3))
     # n = 0, n = 4096 accepted, n = 4097 refused
-    assert lib.xtb_peer_memcpy_batch(*_batch([], [], []), 0, _st()) == 0
+    assert lib.xtb_peer_memcpy_batch(*_batch([], [], []), 0, current_stream()) == 0
     d4 = R.guarded(4096)
     d_ptrs = [d4.ptr(0, i) for i in range(4096)]
     s_ptrs = [src.data_ptr() + 4095 - i for i in range(4096)]
-    _ok(lib.xtb_peer_memcpy_batch(*_batch(d_ptrs, s_ptrs, [1] * 4096), 4096, _st()), "4096 entries")
+    check(lib.xtb_peer_memcpy_batch(*_batch(d_ptrs, s_ptrs, [1] * 4096), 4096, current_stream()), "4096 entries")
     torch.cuda.synchronize()
     assert torch.equal(d4.bytes(0), src[:4096].flip(0))
-    assert lib.xtb_peer_memcpy_batch(*_batch(d_ptrs + d_ptrs[:1], s_ptrs + s_ptrs[:1], [1] * 4097), 4097, _st()) == XTB_ERR_INVALID
+    assert lib.xtb_peer_memcpy_batch(*_batch(d_ptrs + d_ptrs[:1], s_ptrs + s_ptrs[:1], [1] * 4097), 4097,
+                                     current_stream()) == XTB_ERR_INVALID
 
 
 @pytest.mark.parametrize("bad", ["null_dst", "null_src", "negative"])
 def test_peer_memcpy_batch_refuses_before_copying(bad):
     """A batch with a bad second entry is refused and copies nothing, not even the good first entry."""
-    lib = _lib()
+    lib = ensure_init()
     src = R.labels(4096, 1)
     d0, d1 = R.guarded(4096), R.guarded(4096)
     dsts = [d0.ptr(0), None if bad == "null_dst" else d1.ptr(0)]
     srcs = [src.data_ptr(), None if bad == "null_src" else src.data_ptr()]
     nb = [4096, -1 if bad == "negative" else 4096]
-    assert lib.xtb_peer_memcpy_batch(*_batch(dsts, srcs, nb), 2, _st()) == XTB_ERR_INVALID
+    assert lib.xtb_peer_memcpy_batch(*_batch(dsts, srcs, nb), 2, current_stream()) == XTB_ERR_INVALID
     torch.cuda.synchronize()
     assert bool((d0.arena == R.FILL32).all()), "the first entry of a refused batch was copied"
     assert bool((d1.arena == R.FILL32).all())
@@ -607,18 +595,19 @@ def test_peer_memcpy_batch_refuses_before_copying(bad):
 
 
 def test_peer_barrier_world1_and_refusals():
-    lib = _lib()
+    lib = ensure_init()
     pads = torch.zeros(64, dtype=torch.int32, device="cuda")
     table = torch.tensor([pads.data_ptr()], dtype=torch.int64, device="cuda")
     n0 = lib.xtb_launch_count()
-    assert lib.xtb_peer_barrier(table.data_ptr(), 0, 1, 0, _st()) == 0  # world = 1: nothing to wait for, nothing launched
-    assert lib.xtb_peer_barrier(table.data_ptr(), 0, 1, 5, _st()) == 0
+    # world = 1: nothing to wait for, nothing launched
+    assert lib.xtb_peer_barrier(table.data_ptr(), 0, 1, 0, current_stream()) == 0
+    assert lib.xtb_peer_barrier(table.data_ptr(), 0, 1, 5, current_stream()) == 0
     assert lib.xtb_launch_count() == n0
-    assert lib.xtb_peer_barrier(None, 0, 1, 0, _st()) == XTB_ERR_INVALID  # null table
-    assert lib.xtb_peer_barrier(table.data_ptr(), 0, 0, 0, _st()) == XTB_ERR_INVALID  # world 0
-    assert lib.xtb_peer_barrier(table.data_ptr(), 1, 1, 0, _st()) == XTB_ERR_INVALID  # rank >= world
-    assert lib.xtb_peer_barrier(table.data_ptr(), -1, 1, 0, _st()) == XTB_ERR_INVALID
-    assert lib.xtb_peer_barrier(table.data_ptr(), 0, 1, -1, _st()) == XTB_ERR_INVALID  # negative channel
+    assert lib.xtb_peer_barrier(None, 0, 1, 0, current_stream()) == XTB_ERR_INVALID  # null table
+    assert lib.xtb_peer_barrier(table.data_ptr(), 0, 0, 0, current_stream()) == XTB_ERR_INVALID  # world 0
+    assert lib.xtb_peer_barrier(table.data_ptr(), 1, 1, 0, current_stream()) == XTB_ERR_INVALID  # rank >= world
+    assert lib.xtb_peer_barrier(table.data_ptr(), -1, 1, 0, current_stream()) == XTB_ERR_INVALID
+    assert lib.xtb_peer_barrier(table.data_ptr(), 0, 1, -1, current_stream()) == XTB_ERR_INVALID  # negative channel
     assert lib.xtb_launch_count() == n0
     torch.cuda.synchronize()
     assert bool((pads == 0).all())
@@ -646,7 +635,8 @@ def test_a2a_pull_past_2g():
     nbytes = inp.numel() * 2
     assert nbytes > 2**31
     o = R.guarded(nbytes)
-    _ok(_lib().xtb_a2a_pull(table.data_ptr(), o.ptr(0), 1, W, *_a2a_args(plan), _st()), "xtb_a2a_pull")
+    check(ensure_init().xtb_a2a_pull(table.data_ptr(), o.ptr(0), 1, W, *_a2a_args(plan), current_stream()),
+          "xtb_a2a_pull")
     torch.cuda.synchronize()
     out = o.buf(0, torch.int16, plan.out_shape)
     assert plan.out_shape == (W * S, 4, 128)
@@ -663,7 +653,7 @@ def test_ep_pulls_past_2g():
     buffer of R rows (1 GiB), so owner 0 receives 2R rows and writes past 2^31 bytes; rank 1's way back reads past it."""
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats()
-    lib, W, E, rb = _lib(), 2, 2, 14336
+    lib, W, E, rb = ensure_init(), 2, 2, 14336
     words, hdr = rb // 4, R.ep_hdr_bytes(E)
     Rr = (1 << 30) // rb + 101
     assert 2 * Rr * rb > 2**31
@@ -679,8 +669,9 @@ def test_ep_pulls_past_2g():
     own_table = torch.tensor([own.data_ptr()] * W, dtype=torch.int64, device="cuda")
     cnt_out = torch.empty(W * E, dtype=torch.int32, device="cuda")
     status = torch.tensor([-1, 0], dtype=torch.int32, device="cuda")
-    _ok(lib.xtb_ep_pull_to_experts(table.data_ptr(), None, cnt_out.data_ptr(), own.data_ptr() + hdr, None, status.data_ptr(), 0,
-                                   W, E, rb, hdr, 2 * Rr, _st()), "xtb_ep_pull_to_experts")
+    check(lib.xtb_ep_pull_to_experts(table.data_ptr(), None, cnt_out.data_ptr(), own.data_ptr() + hdr, None,
+                                     status.data_ptr(), 0, W, E, rb, hdr, 2 * Rr, current_stream()),
+          "xtb_ep_pull_to_experts")
     torch.cuda.synchronize()
     assert cnt_out.tolist() == [Rr, 0, Rr, 0] and status.tolist() == [2 * Rr, 0]
     got = own[hdr // 4 :]
@@ -692,8 +683,8 @@ def test_ep_pulls_past_2g():
     del got
     back = torch.full((Rr * words + 64,), R.FILL32, dtype=torch.int32, device="cuda")
     cnt_dev = _t(np.array([[Rr, 0], [Rr, 0]], dtype=np.int32))
-    _ok(lib.xtb_ep_pull_to_sources(own_table.data_ptr(), cnt_dev.data_ptr(), back.data_ptr(), 1, W, E, rb, hdr, 2 * Rr, Rr, _st()),
-        "xtb_ep_pull_to_sources")
+    check(lib.xtb_ep_pull_to_sources(own_table.data_ptr(), cnt_dev.data_ptr(), back.data_ptr(), 1, W, E, rb, hdr,
+                                     2 * Rr, Rr, current_stream()), "xtb_ep_pull_to_sources")
     torch.cuda.synchronize()
     for a, b in _chunks(Rr, 8192):
         assert torch.equal(back[a * words : b * words].view(-1, words), rows[a:b]), f"returned rows {a}..{b}"

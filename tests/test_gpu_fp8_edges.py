@@ -23,51 +23,35 @@ import torch
 
 from oracle import moe_oracle as O
 from tests import swiglu_fp8_reference as R
+from xtuner_b200._capi import check, current_stream, ensure_init
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HAVE_REF = os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "xtuner", "v1"))
 
 
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi.ensure_init()
-
-
-def _ok(rc, what):
-    from xtuner_b200._capi import check
-
-    check(rc, what)
-
-
-def _st():
-    from xtuner_b200._capi import current_stream
-
-    return current_stream()
-
-
 def tile_quant(x):
     M, K = x.shape
     q = torch.empty(M, K, dtype=torch.uint8, device="cuda")
     s = torch.empty(M, K // 128, dtype=torch.float32, device="cuda")
-    _ok(_lib().xtb_fp8_per_tile_quant(x.data_ptr(), q.data_ptr(), s.data_ptr(), M, K, _st()), "xtb_fp8_per_tile_quant")
+    check(ensure_init().xtb_fp8_per_tile_quant(x.data_ptr(), q.data_ptr(), s.data_ptr(), M, K, current_stream()),
+          "xtb_fp8_per_tile_quant")
     return q, s
 
 
 def block_scales(w):
     nw, dout, din = w.shape
     s = torch.empty(nw, dout // 128, din // 128, dtype=torch.float32, device="cuda")
-    _ok(_lib().xtb_fp8_block_scales(w.data_ptr(), int(w.dtype == torch.float32), nw, dout, din, s.data_ptr(), _st()),
-        "xtb_fp8_block_scales")
+    check(ensure_init().xtb_fp8_block_scales(w.data_ptr(), int(w.dtype == torch.float32), nw, dout, din, s.data_ptr(),
+                                             current_stream()), "xtb_fp8_block_scales")
     return s
 
 
 def block_cast(w, s):
     nw, dout, din = w.shape
     q = torch.empty(nw, dout, din, dtype=torch.uint8, device="cuda")
-    _ok(_lib().xtb_fp8_block_cast(w.data_ptr(), int(w.dtype == torch.float32), nw, dout, din, s.data_ptr(),
-                                  q.data_ptr(), _st()), "xtb_fp8_block_cast")
+    check(ensure_init().xtb_fp8_block_cast(w.data_ptr(), int(w.dtype == torch.float32), nw, dout, din, s.data_ptr(),
+                                           q.data_ptr(), current_stream()), "xtb_fp8_block_cast")
     return q
 
 
@@ -227,7 +211,7 @@ def test_install_fp8_cast_on_the_reference_functions():
     for w in cases:
         s = ref_scales(w)
         want.append((s, [ref_cast(w[i], s[i]) for i in range(w.shape[0])]))
-    _lib()
+    ensure_init()
     plugin.install_fp8_cast()
     try:
         assert fu.cast_to_per_block_fp8_with_scales is not ref_cast

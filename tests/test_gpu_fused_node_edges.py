@@ -15,6 +15,7 @@ Which case reaches which branch of xtuner_b200/fused.py:
 * residual given and absent, hidden_factor 1 and 0.5, GRAD_SINK, T = 0: the moe cases below say which.
 
 The worst |err| / bound per quantity and the module's wall time are printed at the end."""
+import contextlib
 import time
 
 import pytest
@@ -23,25 +24,27 @@ import torch
 from oracle import moe_oracle as O
 from tests import fused_node_reference as FN
 from tests import gemm_reference as G
+from tests.gpu_harness import Worst
 
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda"
-WORST = {}
+WORST = Worst("fused_node_edges")
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _report():
+@contextlib.contextmanager
+def _wall_time():
     t0 = time.time()
     yield
-    for k, v in sorted(WORST.items()):
-        print(f"fused_node_edges: {k}: {v:.4g}")
     print(f"fused_node_edges: wall time {time.time() - t0:.1f} s")
+
+
+_report = WORST.fixture(_wall_time)
 
 
 def _note(r):
     for k, v in r.items():
-        WORST[k] = max(WORST.get(k, 0.0), float(v))
+        WORST.note(k, v)
 
 
 def _gen(seed):

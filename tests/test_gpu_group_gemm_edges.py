@@ -15,48 +15,10 @@ import torch
 
 from oracle import moe_oracle as O
 from tests import gemm_reference as R
+from tests.gpu_harness import XTB_ERR_INVALID, Guarded
+from xtuner_b200._capi import check, current_stream, ensure_init, ptr
 
 pytestmark = pytest.mark.gpu
-
-XTB_ERR_INVALID = 1
-GUARD = 16
-FILL = 0x7FA5  # a bf16 NaN no kernel produces
-
-
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi.ensure_init()
-
-
-def _st():
-    from xtuner_b200._capi import current_stream
-
-    return current_stream()
-
-
-def _p(t):
-    return t.data_ptr()
-
-
-def _ok(rc, what):
-    from xtuner_b200._capi import check
-
-    check(rc, what)
-
-
-def _guarded(rows, cols):
-    """(buffer, view): the view is rows [GUARD, GUARD + rows) of a NaN-filled int16 buffer, as bf16."""
-    buf = torch.full((rows + 2 * GUARD, cols), FILL, dtype=torch.int16, device="cuda")
-    return buf, buf[GUARD : GUARD + rows].view(torch.bfloat16)
-
-
-def _assert_guarded(buf, rows, what):
-    assert bool((buf[:GUARD] == FILL).all() and (buf[GUARD + rows :] == FILL).all()), f"{what}: a guard row was written"
-    unwritten = buf[GUARD : GUARD + rows] == FILL
-    if bool(unwritten.any()):
-        r, c = (int(i) for i in unwritten.nonzero()[0])
-        raise AssertionError(f"{what}: {int(unwritten.sum())} output elements never written; first at row {r}, column {c}")
 
 
 # ---- the C entries -----------------------------------------------------------------------------------------------------
@@ -64,31 +26,34 @@ def _assert_guarded(buf, rows, what):
 
 def nt(x, w, tpe, out):
     E, N, Kd = w.shape
-    return _lib().xtb_group_gemm_nt(_p(x), _p(w), _p(tpe), x.shape[0], N, Kd, E, _p(out), _st())
+    return ensure_init().xtb_group_gemm_nt(ptr(x), ptr(w), ptr(tpe), x.shape[0], N, Kd, E, ptr(out), current_stream())
 
 
 def nn(dy, w, tpe, out):
     E, N, Kd = w.shape
-    return _lib().xtb_group_gemm_nn(_p(dy), _p(w), _p(tpe), dy.shape[0], N, Kd, E, _p(out), _st())
+    return ensure_init().xtb_group_gemm_nn(ptr(dy), ptr(w), ptr(tpe), dy.shape[0], N, Kd, E, ptr(out), current_stream())
 
 
 def swiglu_gemm(x, w13, tpe, h, a):
     E, twoI, Kd = w13.shape
-    return _lib().xtb_group_gemm_nt_swiglu(_p(x), _p(w13), _p(tpe), x.shape[0], twoI // 2, Kd, E, _p(h), _p(a), _st())
+    return ensure_init().xtb_group_gemm_nt_swiglu(ptr(x), ptr(w13), ptr(tpe), x.shape[0], twoI // 2, Kd, E, ptr(h),
+                                                  ptr(a), current_stream())
 
 
 def tn(dy, x, tpe, dw, E):
-    return _lib().xtb_group_gemm_tn(_p(dy), _p(x), _p(tpe), x.shape[0], dy.shape[1], x.shape[1], E, _p(dw), _st())
+    return ensure_init().xtb_group_gemm_tn(ptr(dy), ptr(x), ptr(tpe), x.shape[0], dy.shape[1], x.shape[1], E, ptr(dw),
+                                           current_stream())
 
 
 def tn_pair(dya, xa, dwa, dyb, xb, dwb, tpe, E):
-    return _lib().xtb_group_gemm_tn_pair(_p(dya), _p(xa), dya.shape[1], xa.shape[1], _p(dwa), _p(dyb), _p(xb), dyb.shape[1],
-                                         xb.shape[1], _p(dwb), _p(tpe), xa.shape[0], E, _st())
+    return ensure_init().xtb_group_gemm_tn_pair(ptr(dya), ptr(xa), dya.shape[1], xa.shape[1], ptr(dwa), ptr(dyb),
+                                                ptr(xb), dyb.shape[1], xb.shape[1], ptr(dwb), ptr(tpe), xa.shape[0], E,
+                                                current_stream())
 
 
 def _xtb_swiglu(h):
     a = torch.empty(h.shape[0], h.shape[1] // 2, dtype=torch.bfloat16, device="cuda")
-    _ok(_lib().xtb_swiglu(_p(h), _p(a), h.shape[0], h.shape[1] // 2, _st()), "xtb_swiglu")
+    check(ensure_init().xtb_swiglu(ptr(h), ptr(a), h.shape[0], h.shape[1] // 2, current_stream()), "xtb_swiglu")
     return a
 
 
@@ -138,11 +103,10 @@ def test_nt_exact(case):
     M = sum(counts)
     x = R.rows_operand(counts, Kd, "exact", 1, "cuda")
     w = R.weight_operand(E, N, Kd, "exact", 2, "cuda")
-    buf, out = _guarded(M, N)
-    _ok(nt(x, w, _tpe(counts), out), "nt")
+    out = Guarded(M, N, torch.bfloat16)
+    check(nt(x, w, _tpe(counts), out.v), "nt")
     torch.cuda.synchronize()
-    _assert_guarded(buf, M, f"nt {case}")
-    R.assert_exact(out, "nt", x, w, counts, f"{case}")
+    R.assert_exact(out.check(f"nt {case}"), "nt", x, w, counts, f"{case}")
 
 
 @pytest.mark.parametrize("case", NN_TN_CASES, ids=_id)
@@ -152,11 +116,10 @@ def test_nn_exact(case):
     M = sum(counts)
     dy = R.rows_operand(counts, N, "exact", 3, "cuda")
     w = R.weight_operand(E, N, Kd, "exact", 4, "cuda")
-    buf, out = _guarded(M, Kd)
-    _ok(nn(dy, w, _tpe(counts), out), "nn")
+    out = Guarded(M, Kd, torch.bfloat16)
+    check(nn(dy, w, _tpe(counts), out.v), "nn")
     torch.cuda.synchronize()
-    _assert_guarded(buf, M, f"nn {case}")
-    R.assert_exact(out, "nn", dy, w, counts, f"{case}")
+    R.assert_exact(out.check(f"nn {case}"), "nn", dy, w, counts, f"{case}")
 
 
 @pytest.mark.parametrize("case", NN_TN_CASES, ids=_id)
@@ -165,11 +128,10 @@ def test_tn_exact(case):
     counts = _counts(E, pattern, 2)
     dy = R.rows_operand(counts, N, "exact", 5, "cuda")
     x = R.rows_operand(counts, Kd, "exact", 6, "cuda")
-    buf, dw = _guarded(E * N, Kd)
-    _ok(tn(dy, x, _tpe(counts), dw, E), "tn")
+    dw = Guarded(E * N, Kd, torch.bfloat16)
+    check(tn(dy, x, _tpe(counts), dw.v, E), "tn")
     torch.cuda.synchronize()
-    _assert_guarded(buf, E * N, f"tn {case}")
-    R.assert_exact(dw.view(E, N, Kd), "tn", dy, x, counts, f"{case}")
+    R.assert_exact(dw.check(f"tn {case}").view(E, N, Kd), "tn", dy, x, counts, f"{case}")
 
 
 # (E, pattern, N_a, Kd_a, N_b, Kd_b): equal tile widths run as one launch, unequal ones as two
@@ -183,12 +145,10 @@ def test_tn_pair_exact(case):
     counts = _counts(E, pattern, 3)
     dya, xa = R.rows_operand(counts, Na, "exact", 7, "cuda"), R.rows_operand(counts, Ka, "exact", 8, "cuda")
     dyb, xb = R.rows_operand(counts, Nb, "exact", 9, "cuda"), R.rows_operand(counts, Kb, "exact", 10, "cuda")
-    bufa, dwa = _guarded(E * Na, Ka)
-    bufb, dwb = _guarded(E * Nb, Kb)
-    _ok(tn_pair(dya, xa, dwa, dyb, xb, dwb, _tpe(counts), E), "tn_pair")
+    ga, gb = Guarded(E * Na, Ka, torch.bfloat16), Guarded(E * Nb, Kb, torch.bfloat16)
+    check(tn_pair(dya, xa, ga.v, dyb, xb, gb.v, _tpe(counts), E), "tn_pair")
     torch.cuda.synchronize()
-    _assert_guarded(bufa, E * Na, f"tn_pair a {case}")
-    _assert_guarded(bufb, E * Nb, f"tn_pair b {case}")
+    dwa, dwb = ga.check(f"tn_pair a {case}"), gb.check(f"tn_pair b {case}")
     R.assert_exact(dwa.view(E, Na, Ka), "tn", dya, xa, counts, f"pair a {case}")
     R.assert_exact(dwb.view(E, Nb, Kb), "tn", dyb, xb, counts, f"pair b {case}")
 
@@ -206,12 +166,10 @@ def test_nt_swiglu_exact(case):
     M = sum(counts)
     x = R.rows_operand(counts, Kd, "exact", 11, "cuda")
     w13 = R.weight_operand(E, 2 * I, Kd, "exact", 12, "cuda")
-    hbuf, h = _guarded(M, 2 * I)
-    abuf, a = _guarded(M, I)
-    _ok(swiglu_gemm(x, w13, _tpe(counts), h, a), "nt_swiglu")
+    hg, ag = Guarded(M, 2 * I, torch.bfloat16), Guarded(M, I, torch.bfloat16)
+    check(swiglu_gemm(x, w13, _tpe(counts), hg.v, ag.v), "nt_swiglu")
     torch.cuda.synchronize()
-    _assert_guarded(hbuf, M, f"nt_swiglu h {case}")
-    _assert_guarded(abuf, M, f"nt_swiglu a {case}")
+    h, a = hg.check(f"nt_swiglu h {case}"), ag.check(f"nt_swiglu a {case}")
     R.assert_exact(h, "nt", x, w13, counts, f"swiglu h {case}")
     _assert_swiglu_a(a, h, f"swiglu {case}")
 
@@ -228,8 +186,8 @@ def test_nt_swiglu_h_is_the_plain_nt_product(I):
     h = torch.empty(M, 2 * I, dtype=torch.bfloat16, device="cuda")
     a = torch.empty(M, I, dtype=torch.bfloat16, device="cuda")
     h_nt = torch.empty_like(h)
-    _ok(swiglu_gemm(x, w13, tpe, h, a), "nt_swiglu")
-    _ok(nt(x, w13, tpe, h_nt), "nt")
+    check(swiglu_gemm(x, w13, tpe, h, a), "nt_swiglu")
+    check(nt(x, w13, tpe, h_nt), "nt")
     torch.cuda.synchronize()
     diff = h.view(torch.int16) != h_nt.view(torch.int16)
     if bool(diff.any()):
@@ -243,7 +201,7 @@ def test_nt_swiglu_h_is_the_plain_nt_product(I):
 def test_more_than_1024_experts_is_rejected():
     """kMaxExperts = 1024 sizes the kernel's shared-memory prefix tables: E = 1025 is refused by every entry, before any
     launch and without touching the output."""
-    lib = _lib()
+    lib = ensure_init()
     E, M = 1025, 128
     counts = [0] * E
     counts[3] = M
@@ -284,32 +242,32 @@ def _expert_mlp_bounds(counts, H, I, seed):
     dy = R.rows_operand(counts, H, "random", seed + 3, "cuda", exp_range=(-4, 0))
     ratios = {}
     h, a = torch.empty(M, 2 * I, **bf), torch.empty(M, I, **bf)
-    _ok(swiglu_gemm(x, w13, tpe, h, a), "nt_swiglu")
+    check(swiglu_gemm(x, w13, tpe, h, a), "nt_swiglu")
     ratios["nt_swiglu.h"] = R.check_bound(h, "nt", x, w13, counts, what="h")
     _assert_swiglu_a(a, h, "production a")
     y = torch.empty(M, H, **bf)
-    _ok(nt(a, w2, tpe, y), "nt")
+    check(nt(a, w2, tpe, y), "nt")
     ratios["nt"] = R.check_bound(y, "nt", a, w2, counts, what="y")
     del y
     da = torch.empty(M, I, **bf)
-    _ok(nn(dy, w2, tpe, da), "nn w2")
+    check(nn(dy, w2, tpe, da), "nn w2")
     ratios["nn.w2"] = R.check_bound(da, "nn", dy, w2, counts, what="da")
     dh = R.rows_operand(counts, 2 * I, "random", seed + 4, "cuda", exp_range=(-4, 0))
     dx = torch.empty(M, H, **bf)
-    _ok(nn(dh, w13, tpe, dx), "nn w13")
+    check(nn(dh, w13, tpe, dx), "nn w13")
     ratios["nn.w13"] = R.check_bound(dx, "nn", dh, w13, counts, what="dx")
     del dx, da
     gw2 = torch.empty(E, H, I, **bf)
-    _ok(tn(dy, a, tpe, gw2, E), "tn")
+    check(tn(dy, a, tpe, gw2, E), "tn")
     ratios["tn"] = R.check_bound(gw2, "tn", dy, a, counts, what="gw2")
     gw2p, gw13p = torch.empty(E, H, I, **bf), torch.empty(E, 2 * I, H, **bf)
-    _ok(tn_pair(dy, a, gw2p, dh, x, gw13p, tpe, E), "tn_pair")
+    check(tn_pair(dy, a, gw2p, dh, x, gw13p, tpe, E), "tn_pair")
     torch.cuda.synchronize()
     assert torch.equal(gw2p.view(torch.int16), gw2.view(torch.int16)), "tn_pair differs from tn (gw2)"
     del gw2, gw2p
     ratios["tn_pair"] = R.check_bound(gw13p, "tn", dh, x, counts, what="gw13 pair")
     gw13 = torch.empty(E, 2 * I, H, **bf)
-    _ok(tn(dh, x, tpe, gw13, E), "tn w13")
+    check(tn(dh, x, tpe, gw13, E), "tn w13")
     torch.cuda.synchronize()
     assert torch.equal(gw13p.view(torch.int16), gw13.view(torch.int16)), "tn_pair differs from tn (gw13)"
     del gw13, gw13p
@@ -345,9 +303,9 @@ def test_bound_128_experts_and_ops_group_gemm():
     da, dw = torch.autograd.grad(y, (ar, wr), dy)
     bf = dict(dtype=torch.bfloat16, device="cuda")
     y_c, da_c, dw_c = torch.empty_like(y), torch.empty(a.shape, **bf), torch.empty(w2.shape, **bf)
-    _ok(nt(a, w2, tpe, y_c), "nt")
-    _ok(nn(dy, w2, tpe, da_c), "nn")
-    _ok(tn(dy, a, tpe, dw_c, 128), "tn")
+    check(nt(a, w2, tpe, y_c), "nt")
+    check(nn(dy, w2, tpe, da_c), "nn")
+    check(tn(dy, a, tpe, dw_c, 128), "tn")
     torch.cuda.synchronize()
     for got, want in ((y, y_c), (da, da_c), (dw, dw_c)):
         assert torch.equal(got.detach().view(torch.int16), want.view(torch.int16))
@@ -391,22 +349,22 @@ def test_poisoned_neighbours_do_not_reach_the_victim(entry, victim_rows):
         bf = dict(dtype=torch.bfloat16, device="cuda")
         if entry == "nt":
             out = torch.empty(M, N, **bf)
-            _ok(nt(pick(X), pick(W), tpe, out), entry)
+            check(nt(pick(X), pick(W), tpe, out), entry)
             return [out[lo:hi]]
         if entry == "nn":
             out = torch.empty(M, Kd, **bf)
-            _ok(nn(pick(DY), pick(W), tpe, out), entry)
+            check(nn(pick(DY), pick(W), tpe, out), entry)
             return [out[lo:hi]]
         if entry == "nt_swiglu":
             h, a = torch.empty(M, 2 * I, **bf), torch.empty(M, I, **bf)
-            _ok(swiglu_gemm(pick(X), pick(W13), tpe, h, a), entry)
+            check(swiglu_gemm(pick(X), pick(W13), tpe, h, a), entry)
             return [h[lo:hi], a[lo:hi]]
         if entry == "tn":
             dw = torch.empty(E, N, Kd, **bf)
-            _ok(tn(pick(DY), pick(X), tpe, dw, E), entry)
+            check(tn(pick(DY), pick(X), tpe, dw, E), entry)
             return [dw[VICTIM], dw[1], dw[6]]
         dwa, dwb = torch.empty(E, N, Kd, **bf), torch.empty(E, 2 * I, Kd, **bf)
-        _ok(tn_pair(pick(DY), pick(X), dwa, pick(DH), pick(X), dwb, tpe, E), entry)
+        check(tn_pair(pick(DY), pick(X), dwa, pick(DH), pick(X), dwb, tpe, E), entry)
         return [dwa[VICTIM], dwb[VICTIM], dwa[1], dwb[6]]
 
     X, DY, DH = rows(Kd, 31), rows(N, 32), rows(2 * I, 33)
@@ -428,7 +386,7 @@ def test_ops_group_gemm_rejects_inconsistent_shapes_before_launching():
     from xtuner_b200 import ops
     from xtuner_b200._capi import XtbError
 
-    lib = _lib()
+    lib = ensure_init()
     bf = dict(dtype=torch.bfloat16, device="cuda")
     x = torch.randn(300, 256, **bf)
     w = torch.randn(4, 128, 256, **bf)

@@ -33,95 +33,43 @@
 Every output is written into a view with 16 guard rows on each side (the workspace: 16 pairs after its T * n_vt pairs),
 pre-filled with a NaN pattern no kernel produces: the guards must keep the fill and no output element may keep it.  Each
 quantity's worst |err| / bound and each V's exact share of G are printed at the end of the module."""
+import contextlib
 import math
 
 import pytest
 import torch
 
 from tests import gemm_reference as R
+from tests.gpu_harness import FILL32, GUARD, Guarded, Worst
 from tests.lm_head_ce_reference import grad64, lm_head_ce, logp64, logprob_grad64, row_ce64, row_stats64
+from xtuner_b200._capi import check, current_stream, ensure_init, ptr
 
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda"
 IGN = -100
-GUARD = 16
-FILL16 = 0x7FA5  # a bf16 NaN no kernel produces
-FILL32 = 0x7FC0A5A5  # an fp32 NaN no kernel produces
 WS_HEADER = 256  # bytes of the workspace ahead of its tile pairs
 REL = 1e-6  # CE, logp and log-sum: relative to max(1, |value|)
 # the loss: each row's CE within REL, the products rounded once, and an fp32 sum of at most 40 dependent adds (one term
 # per thread below 1024 rows, a 5-level warp butterfly, 32 warp results in order)
 LOSS_REL = REL + 40 * 2.0 ** -24
-WORST = {}  # quantity -> largest |err| / bound seen
+WORST = Worst("lm_head_edges")
 SHARE = {}  # case -> exact share of G
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _report():
+@contextlib.contextmanager
+def _shares():
     yield
-    for k, v in sorted(WORST.items()):
-        print(f"lm_head_edges: {k}: {v:.4g}")
     for k, v in SHARE.items():
         print(f"lm_head_edges: G exact share {k}: {v:.6f}")
 
 
-def _note(name, r):
-    WORST[name] = max(WORST.get(name, 0.0), float(r))
-
-
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi.ensure_init()
-
-
-def _st():
-    from xtuner_b200._capi import current_stream
-
-    return current_stream()
-
-
-def _p(t):
-    return None if t is None else t.data_ptr()
-
-
-def _ok(rc, what):
-    from xtuner_b200._capi import check
-
-    check(rc, what)
-
-
-def _guarded(rows, cols, fp32=False):
-    """(buffer, view): rows [GUARD, GUARD + rows) of a NaN-filled integer buffer, as bf16 (or fp32)."""
-    if fp32:
-        buf = torch.full((rows + 2 * GUARD, cols), FILL32, dtype=torch.int32, device=DEV)
-        return buf, buf[GUARD:GUARD + rows].view(torch.float32)
-    buf = torch.full((rows + 2 * GUARD, cols), FILL16, dtype=torch.int16, device=DEV)
-    return buf, buf[GUARD:GUARD + rows].view(torch.bfloat16)
-
-
-def _fill(buf):
-    return FILL32 if buf.dtype == torch.int32 else FILL16
-
-
-def _assert_guarded(buf, rows, what):
-    """Guard rows keep the fill and every element of the rows in between was written."""
-    fill = _fill(buf)
-    assert bool((buf[:GUARD] == fill).all() and (buf[GUARD + rows:] == fill).all()), f"{what}: a guard row was written"
-    miss = buf[GUARD:GUARD + rows] == fill
-    if bool(miss.any()):
-        r, c = (int(i) for i in miss.nonzero()[0])
-        raise AssertionError(f"{what}: {int(miss.sum())} output elements never written; first at row {r}, column {c}")
-
-
-def _untouched(buf, what):
-    assert bool((buf == _fill(buf)).all()), f"{what}: written, but nothing should have been"
+_report = WORST.fixture(_shares)
 
 
 def _workspace(T, V):
     """int32 workspace of xtb_lm_head_ce_workspace_bytes(T, V) bytes plus 16 guard pairs, all filled"""
-    n = int(_lib().xtb_lm_head_ce_workspace_bytes(T, V))
+    n = int(ensure_init().xtb_lm_head_ce_workspace_bytes(T, V))
     assert n % 8 == 0
     return n, torch.full((n // 4 + 2 * GUARD,), FILL32, dtype=torch.int32, device=DEV)
 
@@ -151,23 +99,17 @@ def ce(h, w, lab, lw, need_grad, ignore=IGN):
     T, H = h.shape
     V = w.shape[0]
     o = Out()
-    zb, o.z = _guarded(T, V)
-    cb, c = _guarded(T, 1, fp32=True)
-    lb, l = _guarded(1, 1, fp32=True)
-    dhb, o.dh = _guarded(T, H) if need_grad else (None, None)
-    dwb, o.dw = _guarded(V, H) if need_grad else (None, None)
+    z, c, l = Guarded(T, V, torch.bfloat16), Guarded(T, 1, torch.float32), Guarded(1, 1, torch.float32)
+    dh, dw = (Guarded(T, H, torch.bfloat16), Guarded(V, H, torch.bfloat16)) if need_grad else (None, None)
     n, ws = _workspace(T, V)
-    _ok(_lib().xtb_lm_head_ce(_p(h), _p(w), _p(lab), _p(lw), T, H, V, ignore, int(need_grad), _p(o.z), _p(ws), _p(c),
-                              _p(l), _p(o.dh), _p(o.dw), _st()), "xtb_lm_head_ce")
+    check(ensure_init().xtb_lm_head_ce(ptr(h), ptr(w), ptr(lab), ptr(lw), T, H, V, ignore, int(need_grad), ptr(z.v),
+                                       ptr(ws), ptr(c.v), ptr(l.v), ptr(dh.v) if need_grad else None,
+                                       ptr(dw.v) if need_grad else None, current_stream()), "xtb_lm_head_ce")
     torch.cuda.synchronize()
-    _assert_guarded(zb, T, "z / G")
-    _assert_guarded(cb, T, "row_ce")
-    _assert_guarded(lb, 1, "loss")
-    if need_grad:
-        _assert_guarded(dhb, T, "dh")
-        _assert_guarded(dwb, V, "dW")
+    o.z, o.ce, o.loss = z.check("z / G"), c.check("row_ce")[:, 0], l.check("loss")[0, 0]
+    o.dh, o.dw = (dh.check("dh"), dw.check("dW")) if need_grad else (None, None)
     _check_ws(n, ws, T, V, "xtb_lm_head_ce workspace")
-    o.ce, o.loss, o.pairs = c[:, 0], l[0, 0], _pairs(ws, T, V)
+    o.pairs = _pairs(ws, T, V)
     return o
 
 
@@ -176,18 +118,14 @@ def logprob(h, w, lab):
     T, H = h.shape
     V = w.shape[0]
     o = Out()
-    zb, o.z = _guarded(T, V)
-    pb, lp = _guarded(T, 1, fp32=True)
-    rb, o.rs = _guarded(T, 2, fp32=True)
+    z, lp, rs = Guarded(T, V, torch.bfloat16), Guarded(T, 1, torch.float32), Guarded(T, 2, torch.float32)
     n, ws = _workspace(T, V)
-    _ok(_lib().xtb_lm_head_logprob(_p(h), _p(w), _p(lab), T, H, V, _p(o.z), _p(ws), _p(lp), _p(o.rs), _st()),
-        "xtb_lm_head_logprob")
+    check(ensure_init().xtb_lm_head_logprob(ptr(h), ptr(w), ptr(lab), T, H, V, ptr(z.v), ptr(ws), ptr(lp.v), ptr(rs.v),
+                                            current_stream()), "xtb_lm_head_logprob")
     torch.cuda.synchronize()
-    _assert_guarded(zb, T, "logprob z")
-    _assert_guarded(pb, T, "logp")
-    _assert_guarded(rb, T, "row_stats")
+    o.z, o.logp, o.rs = z.check("logprob z"), lp.check("logp")[:, 0], rs.check("row_stats")
     _check_ws(n, ws, T, V, "xtb_lm_head_logprob workspace")
-    o.logp, o.pairs = lp[:, 0], _pairs(ws, T, V)
+    o.pairs = _pairs(ws, T, V)
     return o
 
 
@@ -195,28 +133,24 @@ def logprob_bwd(z, rs, lab, c, h, w):
     """one xtb_lm_head_logprob_bwd call over z (a guarded view, overwritten with G) -> (dh, dW)"""
     T, H = h.shape
     V = w.shape[0]
-    dhb, dh = _guarded(T, H)
-    dwb, dw = _guarded(V, H)
+    dh, dw = Guarded(T, H, torch.bfloat16), Guarded(V, H, torch.bfloat16)
     n, ws = _workspace(0, V)
-    _ok(_lib().xtb_lm_head_logprob_bwd(_p(z), _p(rs), _p(lab), _p(c), _p(h), _p(w), T, H, V, _p(ws), _p(dh), _p(dw),
-                                       _st()), "xtb_lm_head_logprob_bwd")
+    check(ensure_init().xtb_lm_head_logprob_bwd(ptr(z), ptr(rs), ptr(lab), ptr(c), ptr(h), ptr(w), T, H, V, ptr(ws),
+                                                ptr(dh.v), ptr(dw.v), current_stream()), "xtb_lm_head_logprob_bwd")
     torch.cuda.synchronize()
-    _assert_guarded(dhb, T, "logprob dh")
-    _assert_guarded(dwb, V, "logprob dW")
     assert bool((ws[n // 4:] == FILL32).all()), "logprob_bwd: written past the workspace"
-    return dh, dw
+    return dh.check("logprob dh"), dw.check("logprob dW")
 
 
 def gemm(kind, a, b, T):
     """xtb_group_gemm_nn (a = G [T, V], b = w [V, H] -> [T, H]) or _tn (a = G, b = h [T, H] -> [V, H]), one group"""
     V, H = a.shape[1], b.shape[1]
     tpe = torch.tensor([T], dtype=torch.int64, device=DEV)
-    buf, out = _guarded(T if kind == "nn" else V, H)
-    f = _lib().xtb_group_gemm_nn if kind == "nn" else _lib().xtb_group_gemm_tn
-    _ok(f(_p(a), _p(b), _p(tpe), T, V, H, 1, _p(out), _st()), f"xtb_group_gemm_{kind}")
+    out = Guarded(T if kind == "nn" else V, H, torch.bfloat16)
+    f = ensure_init().xtb_group_gemm_nn if kind == "nn" else ensure_init().xtb_group_gemm_tn
+    check(f(ptr(a), ptr(b), ptr(tpe), T, V, H, 1, ptr(out.v), current_stream()), f"xtb_group_gemm_{kind}")
     torch.cuda.synchronize()
-    _assert_guarded(buf, out.shape[0], f"{kind} output")
-    return out
+    return out.check(f"{kind} output")
 
 
 def _labels(T, V, seed, ignored=0.3, ign=IGN):
@@ -244,7 +178,7 @@ def _rel(got, want, name, rows=None):
         got, want = got[rows], want[rows]
     r = ((got.double() - want).abs() / want.abs().clamp_min(1.0)).nan_to_num(math.inf) / REL
     if r.numel():
-        _note(name, r.max())
+        WORST.note(name, r.max())
         assert float(r.max()) <= 1.0, f"{name}: error {float(r.max()) * REL:.3g} relative, row {int(r.argmax())}"
 
 
@@ -255,7 +189,7 @@ def _ulp(G, g64, name, share_key=None, rows=None):
         G, g64 = G[rows], g64[rows]
     d = R.ulp_distance(G, R.bf16_rn(g64))
     share = (d == 0).double().mean().item()
-    _note(f"{name} max ulp (bound 1)", d.max())
+    WORST.note(f"{name} max ulp (bound 1)", d.max())
     if share_key is not None:
         SHARE[share_key] = min(share, SHARE.get(share_key, 1.0))
     assert int(d.max()) <= 1, f"{name}: {int((d > 1).sum())} elements more than 1 ulp from bf16(fp64)"
@@ -270,14 +204,14 @@ def _check_pairs(pairs, z, what):
     assert torch.equal(pairs[..., 0].double(), m), f"{what}: a tile max differs"
     s = torch.exp(zt - m[..., None]).sum(2)
     r = (pairs[..., 1].double() - s).abs() / (s * _width(V) * 2.0 ** -23)
-    _note("tile sum exp / bound", r.max())
+    WORST.note("tile sum exp / bound", r.max())
     assert float(r.max()) <= 1.0, f"{what}: tile sum off by {float(r.max())} x its bound"
 
 
 def _check_loss(loss, ce64, lw, name="loss / bound"):
     prod = ce64 * lw.double()
     r = abs(loss.item() - prod.sum().item()) / (LOSS_REL * prod.abs().sum().item())
-    _note(name, r)
+    WORST.note(name, r)
     assert r <= 1.0, f"loss {loss.item()!r} against fp64 {prod.sum().item()!r}"
 
 
@@ -570,44 +504,39 @@ def test_zero_rows_at_the_entries_write_only_their_contract():
     h, w = _random(1, H, V, seed=79)
     lab = torch.zeros(1, dtype=torch.int64, device=DEV)
     lw = torch.ones(1, device=DEV)
-    lib = _lib()
+    lib = ensure_init()
     for need_grad in (1, 0):  # one row of every buffer, so that no pointer is NULL
-        zb, z = _guarded(1, V)
-        cb, c = _guarded(1, 1, fp32=True)
-        lb, l = _guarded(1, 1, fp32=True)
-        dhb, dh = _guarded(1, H)
-        dwb, dw = _guarded(V, H)
+        z, c, l = Guarded(1, V, torch.bfloat16), Guarded(1, 1, torch.float32), Guarded(1, 1, torch.float32)
+        dh, dw = Guarded(1, H, torch.bfloat16), Guarded(V, H, torch.bfloat16)
         wsb = torch.full((1024,), FILL32, dtype=torch.int32, device=DEV)
-        _ok(lib.xtb_lm_head_ce(_p(h), _p(w), _p(lab), _p(lw), 0, H, V, IGN, need_grad, _p(z), _p(wsb), _p(c), _p(l),
-                               _p(dh), _p(dw), _st()), "xtb_lm_head_ce")
+        check(lib.xtb_lm_head_ce(ptr(h), ptr(w), ptr(lab), ptr(lw), 0, H, V, IGN, need_grad, ptr(z.v), ptr(wsb),
+                                 ptr(c.v), ptr(l.v), ptr(dh.v), ptr(dw.v), current_stream()), "xtb_lm_head_ce")
         torch.cuda.synchronize()
-        assert l.view(torch.int32)[0, 0].item() == 0, "the loss is not +0"
-        for b, name in ((zb, "z"), (cb, "row_ce"), (dhb, "dh"), (wsb, "workspace")):
-            _untouched(b, f"T = 0, need_grad {need_grad}: {name}")
-        assert bool((lb[:GUARD] == FILL32).all() and (lb[GUARD + 1:] == FILL32).all())
+        what = f"T = 0, need_grad {need_grad}"
+        assert l.check(f"{what}: loss", written=None).view(torch.int32)[0, 0].item() == 0, "the loss is not +0"
+        for g, name in ((z, "z"), (c, "row_ce"), (dh, "dh")):
+            g.check(f"{what}: {name}", written=False)
+        assert bool((wsb == FILL32).all()), f"{what}: workspace written"
         if need_grad:
-            assert bool((dw.view(torch.int16) == 0).all()) and bool((dwb[:GUARD] == FILL16).all())
-            assert bool((dwb[GUARD + V:] == FILL16).all())
+            assert bool((dw.check(f"{what}: dW", written=None).view(torch.int16) == 0).all())
         else:
-            _untouched(dwb, "T = 0 without grad: dW")
-    zb, z = _guarded(1, V)
-    pb, lp = _guarded(1, 1, fp32=True)
-    rb, rs = _guarded(1, 2, fp32=True)
+            dw.check(f"{what}: dW", written=False)
+    z, lp, rs = Guarded(1, V, torch.bfloat16), Guarded(1, 1, torch.float32), Guarded(1, 2, torch.float32)
     wsb = torch.full((1024,), FILL32, dtype=torch.int32, device=DEV)
-    _ok(lib.xtb_lm_head_logprob(_p(h), _p(w), _p(lab), 0, H, V, _p(z), _p(wsb), _p(lp), _p(rs), _st()),
-        "xtb_lm_head_logprob")
+    check(lib.xtb_lm_head_logprob(ptr(h), ptr(w), ptr(lab), 0, H, V, ptr(z.v), ptr(wsb), ptr(lp.v), ptr(rs.v),
+                                  current_stream()), "xtb_lm_head_logprob")
     torch.cuda.synchronize()
-    for b, name in ((zb, "z"), (pb, "logp"), (rb, "row_stats"), (wsb, "workspace")):
-        _untouched(b, f"logprob T = 0: {name}")
-    dhb, dh = _guarded(1, H)
-    dwb, dw = _guarded(V, H)
-    _ok(lib.xtb_lm_head_logprob_bwd(_p(z), _p(rs), _p(lab), _p(lw), _p(h), _p(w), 0, H, V, _p(wsb), _p(dh), _p(dw),
-                                    _st()), "xtb_lm_head_logprob_bwd")
+    for g, name in ((z, "z"), (lp, "logp"), (rs, "row_stats")):
+        g.check(f"logprob T = 0: {name}", written=False)
+    assert bool((wsb == FILL32).all()), "logprob T = 0: workspace written"
+    dh, dw = Guarded(1, H, torch.bfloat16), Guarded(V, H, torch.bfloat16)
+    check(lib.xtb_lm_head_logprob_bwd(ptr(z.v), ptr(rs.v), ptr(lab), ptr(lw), ptr(h), ptr(w), 0, H, V, ptr(wsb),
+                                      ptr(dh.v), ptr(dw.v), current_stream()), "xtb_lm_head_logprob_bwd")
     torch.cuda.synchronize()
-    for b, name in ((zb, "z"), (rb, "row_stats"), (dhb, "dh"), (wsb, "workspace")):
-        _untouched(b, f"logprob_bwd T = 0: {name}")
-    assert bool((dw.view(torch.int16) == 0).all()) and bool((dwb[:GUARD] == FILL16).all())
-    assert bool((dwb[GUARD + V:] == FILL16).all())
+    for g, name in ((z, "z"), (rs, "row_stats"), (dh, "dh")):
+        g.check(f"logprob_bwd T = 0: {name}", written=False)
+    assert bool((wsb == FILL32).all()), "logprob_bwd T = 0: workspace written"
+    assert bool((dw.check("logprob_bwd T = 0: dW", written=None).view(torch.int16) == 0).all())
 
 
 @pytest.mark.parametrize("chunk", [None, 1024])

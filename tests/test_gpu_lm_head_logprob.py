@@ -14,6 +14,7 @@ import torch
 from torch.nn import functional as F
 
 from tests import gemm_reference as R
+from xtuner_b200._capi import check, current_stream, ensure_init, ptr
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,50 +23,41 @@ DEV = "cuda"
 IGN = -100
 
 
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi, _capi.ensure_init()
-
-
 def _fwd(h, w, lab, z, stats=True):
     """one xtb_lm_head_logprob call -> (logp, row_stats or None); z receives the logits"""
-    _capi, lib = _lib()
+    lib = ensure_init()
     T, H = h.shape
     V = w.shape[0]
     ws = torch.empty(max(int(lib.xtb_lm_head_logprob_workspace_bytes(T, V)), 16), dtype=torch.uint8, device=DEV)
     logp = torch.empty(T, dtype=torch.float32, device=DEV)
     rs = torch.empty((T, 2), dtype=torch.float32, device=DEV) if stats else None
-    p = _capi.ptr
-    _capi.check(lib.xtb_lm_head_logprob(p(h), p(w), p(lab), T, H, V, p(z), p(ws), p(logp), p(rs), _capi.current_stream()),
-                "xtb_lm_head_logprob")
+    check(lib.xtb_lm_head_logprob(ptr(h), ptr(w), ptr(lab), T, H, V, ptr(z), ptr(ws), ptr(logp), ptr(rs),
+                                  current_stream()), "xtb_lm_head_logprob")
     return logp, rs
 
 
 def _bwd(z, rs, lab, c, h, w):
     """one xtb_lm_head_logprob_bwd call -> (dh, dW); z receives G"""
-    _capi, lib = _lib()
+    lib = ensure_init()
     T, H = h.shape
     V = w.shape[0]
     ws = torch.empty(max(int(lib.xtb_lm_head_logprob_workspace_bytes(0, V)), 16), dtype=torch.uint8, device=DEV)
     dh, dw = torch.empty_like(h), torch.empty_like(w)
-    p = _capi.ptr
-    _capi.check(lib.xtb_lm_head_logprob_bwd(p(z), p(rs), p(lab), p(c), p(h), p(w), T, H, V, p(ws), p(dh), p(dw),
-                                            _capi.current_stream()), "xtb_lm_head_logprob_bwd")
+    check(lib.xtb_lm_head_logprob_bwd(ptr(z), ptr(rs), ptr(lab), ptr(c), ptr(h), ptr(w), T, H, V, ptr(ws), ptr(dh),
+                                      ptr(dw), current_stream()), "xtb_lm_head_logprob_bwd")
     return dh, dw
 
 
 def _ce(h, w, lab, lw, z):
-    _capi, lib = _lib()
+    lib = ensure_init()
     T, H = h.shape
     V = w.shape[0]
     ws = torch.empty(max(int(lib.xtb_lm_head_ce_workspace_bytes(T, V)), 16), dtype=torch.uint8, device=DEV)
     row_ce = torch.empty(T, dtype=torch.float32, device=DEV)
     loss = torch.empty((), dtype=torch.float32, device=DEV)
     dh, dw = torch.empty_like(h), torch.empty_like(w)
-    p = _capi.ptr
-    _capi.check(lib.xtb_lm_head_ce(p(h), p(w), p(lab), p(lw), T, H, V, IGN, 1, p(z), p(ws), p(row_ce), p(loss), p(dh),
-                                   p(dw), _capi.current_stream()), "xtb_lm_head_ce")
+    check(lib.xtb_lm_head_ce(ptr(h), ptr(w), ptr(lab), ptr(lw), T, H, V, IGN, 1, ptr(z), ptr(ws), ptr(row_ce),
+                             ptr(loss), ptr(dh), ptr(dw), current_stream()), "xtb_lm_head_ce")
     return row_ce, dh, dw
 
 

@@ -11,7 +11,8 @@
 import pytest
 import torch
 
-from tests.test_gpu_swiglu_edges import _assert_guarded, _guarded
+from tests.gpu_harness import Guarded
+from xtuner_b200._capi import check, current_stream, ensure_init
 
 pytestmark = pytest.mark.gpu
 
@@ -21,16 +22,8 @@ C2 = (8192, 2048, 768, 8, 2)
 QWEN3_30B_A3B = (4096, 2048, 768, 128, 8)
 
 
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi.ensure_init()
-
-
 def _call(name, *args):
-    from xtuner_b200._capi import check, current_stream
-
-    check(getattr(_lib(), name)(*args, current_stream()), name)
+    check(getattr(ensure_init(), name)(*args, current_stream()), name)
 
 
 def _bits(t):
@@ -43,17 +36,14 @@ def _bits(t):
 def _swiglu_pair(h, d):
     """(a, g_h) of xtb_swiglu_bwd_act in guarded buffers, and (a, g_h) of xtb_swiglu and xtb_swiglu_bwd"""
     M, I = d.shape
-    abuf, a = _guarded(M, I)
-    gbuf, gh = _guarded(M, 2 * I)
-    _call("xtb_swiglu_bwd_act", d.data_ptr(), h.data_ptr(), gh.data_ptr(), a.data_ptr(), M, I)
+    a, gh = Guarded(M, I, torch.bfloat16), Guarded(M, 2 * I, torch.bfloat16)
+    _call("xtb_swiglu_bwd_act", d.data_ptr(), h.data_ptr(), gh.v.data_ptr(), a.v.data_ptr(), M, I)
     a_ref = torch.empty(M, I, dtype=torch.bfloat16, device=DEV)
     gh_ref = torch.empty(M, 2 * I, dtype=torch.bfloat16, device=DEV)
     _call("xtb_swiglu", h.data_ptr(), a_ref.data_ptr(), M, I)
     _call("xtb_swiglu_bwd", d.data_ptr(), h.data_ptr(), gh_ref.data_ptr(), M, I)
     torch.cuda.synchronize()
-    _assert_guarded(abuf, M, "act")
-    _assert_guarded(gbuf, M, "grad_h")
-    return (a, gh), (a_ref, gh_ref)
+    return (a.check("act"), gh.check("grad_h")), (a_ref, gh_ref)
 
 
 def test_swiglu_bwd_act_at_every_gate_value():

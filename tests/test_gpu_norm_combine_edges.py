@@ -23,78 +23,13 @@ import pytest
 import torch
 
 from tests import norm_combine_reference as R
+from tests.gpu_harness import XTB_ERR_INVALID, Guarded, Worst, sm_count
+from xtuner_b200._capi import check, current_stream, ensure_init, ptr
 
 pytestmark = pytest.mark.gpu
 
-XTB_ERR_INVALID = 1
-GUARD = 16
-FILL16 = 0x7FA5  # a bf16 NaN no kernel produces
-FILL32 = 0x7FC0A5A5  # an fp32 NaN no kernel produces
-WORST = {}  # quantity -> largest |err| / bound seen (printed at the end of the module)
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report():
-    yield
-    for k, v in sorted(WORST.items()):
-        print(f"norm_combine_edges: {k}: {v:.4g}")
-
-
-def _note(name, r):
-    if isinstance(r, tuple):
-        r = r[0]
-    WORST[name] = max(WORST.get(name, 0.0), float(r))
-
-
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi.ensure_init()
-
-
-def _st():
-    from xtuner_b200._capi import current_stream
-
-    return current_stream()
-
-
-def _p(t):
-    return None if t is None else t.data_ptr()
-
-
-def _ok(rc, what):
-    from xtuner_b200._capi import check
-
-    check(rc, what)
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _guarded(rows, cols, fp32=False):
-    """(buffer, view): rows [GUARD, GUARD + rows) of a NaN-filled integer buffer, as bf16 (or fp32)."""
-    if fp32:
-        buf = torch.full((rows + 2 * GUARD, cols), FILL32, dtype=torch.int32, device="cuda")
-        return buf, buf[GUARD : GUARD + rows].view(torch.float32)
-    buf = torch.full((rows + 2 * GUARD, cols), FILL16, dtype=torch.int16, device="cuda")
-    return buf, buf[GUARD : GUARD + rows].view(torch.bfloat16)
-
-
-def _assert_guarded(buf, rows, what, written=None):
-    """Guard rows untouched; every row in ``written`` (all rows if None) fully written, every other row untouched."""
-    fill = FILL32 if buf.dtype == torch.int32 else FILL16
-    assert bool((buf[:GUARD] == fill).all() and (buf[GUARD + rows :] == fill).all()), f"{what}: a guard row was written"
-    unw = buf[GUARD : GUARD + rows] == fill
-    if written is None:
-        written = torch.ones(rows, dtype=torch.bool, device=buf.device)
-    miss = unw & written[:, None]
-    if bool(miss.any()):
-        r, c = (int(i) for i in miss.nonzero()[0])
-        raise AssertionError(f"{what}: {int(miss.sum())} output elements never written; first at row {r}, column {c}")
-    stray = ~unw.all(1) & ~written
-    if bool(stray.any()):
-        raise AssertionError(f"{what}: row {int(stray.nonzero()[0])} is referenced by no entry but was written")
+WORST = Worst("norm_combine_edges")
+_report = WORST.fixture()
 
 
 # ---- the C entries -----------------------------------------------------------------------------------------------------
@@ -102,28 +37,31 @@ def _assert_guarded(buf, rows, what, written=None):
 
 def combine(y, rmap, p, res, hf, T, K, H, out):
     if res is None and hf == 1.0:
-        return _lib().xtb_moe_unpermute(_p(y), _p(rmap), _p(p), T, K, H, _p(out), _st())
-    return _lib().xtb_moe_combine(_p(y), _p(rmap), _p(p), _p(res), hf, T, K, H, _p(out), _st())
+        return ensure_init().xtb_moe_unpermute(ptr(y), ptr(rmap), ptr(p), T, K, H, ptr(out), current_stream())
+    return ensure_init().xtb_moe_combine(ptr(y), ptr(rmap), ptr(p), ptr(res), hf, T, K, H, ptr(out), current_stream())
 
 
 def unpermute_bwd(g, y, rmap, p, T, K, H, act, pg):
-    return _lib().xtb_moe_unpermute_bwd(_p(g), _p(y), _p(rmap), _p(p), T, K, H, _p(act), _p(pg), _st())
+    return ensure_init().xtb_moe_unpermute_bwd(ptr(g), ptr(y), ptr(rmap), ptr(p), T, K, H, ptr(act), ptr(pg),
+                                               current_stream())
 
 
 def rmsnorm_gate(h, w, gate_w, T, H, E, x, rstd, logits, eps=R.EPS):
-    return _lib().xtb_rmsnorm_gate(_p(h), _p(w), _p(gate_w), eps, T, H, E, _p(x), _p(rstd), _p(logits), _st())
+    return ensure_init().xtb_rmsnorm_gate(ptr(h), ptr(w), ptr(gate_w), eps, T, H, E, ptr(x), ptr(rstd), ptr(logits),
+                                          current_stream())
 
 
 def dispatch_bwd(g_xp, rmap, gate, h, rstd, w, g_res, T, K, H, g_h, g_nw):
+    lib = ensure_init()
     ws = None
     if g_nw is not None:
-        ws = torch.empty(int(_lib().xtb_moe_dispatch_bwd_rmsnorm_workspace_bytes(T, H)), dtype=torch.uint8, device="cuda")
-    return _lib().xtb_moe_dispatch_bwd_rmsnorm(_p(g_xp), _p(rmap), _p(gate), _p(h), _p(rstd), _p(w), _p(g_res), T, K, H,
-                                               _p(g_h), _p(g_nw), _p(ws), _st())
+        ws = torch.empty(int(lib.xtb_moe_dispatch_bwd_rmsnorm_workspace_bytes(T, H)), dtype=torch.uint8, device="cuda")
+    return lib.xtb_moe_dispatch_bwd_rmsnorm(ptr(g_xp), ptr(rmap), ptr(gate), ptr(h), ptr(rstd), ptr(w), ptr(g_res), T,
+                                            K, H, ptr(g_h), ptr(g_nw), ptr(ws), current_stream())
 
 
 def _n_cta(T):
-    return max(1, min(2 * _sms(), (T + 3) // 4))
+    return max(1, min(2 * sm_count(), (T + 3) // 4))
 
 
 # ---- combine / unpermute -----------------------------------------------------------------------------------------------
@@ -139,15 +77,15 @@ def _combine_case(K, H, T, mode, with_p, with_res, hf, seed):
     y = R.permuted_rows(owner, H, sc, mode, seed + 2)  # rows no entry references are NaN
     p = R.probs(T, K, mode, seed + 3, "cuda") if with_p else None
     res = R.token_rows(sc, H, "random", seed + 4) if with_res else None
-    buf, out = _guarded(T, H)
-    _ok(combine(y, rmap, p, res, hf, T, K, H, out), "combine")
+    out = Guarded(T, H, torch.bfloat16)
+    check(combine(y, rmap, p, res, hf, T, K, H, out.v), "combine")
     torch.cuda.synchronize()
     what = f"combine K={K} H={H} T={T} {mode} probs={with_p} residual={with_res} hf={hf}"
-    _assert_guarded(buf, T, what)
+    out.check(what)
     want = R.combine(y, rmap, p, res, hf, K)
-    R.assert_bits_equal(out, want, what)
+    R.assert_bits_equal(out.v, want, what)
     ref, bnd = R.combine_ref(y, rmap, p, res, hf, K)
-    _note("combine restatement vs fp64", R.check_bound(want, ref, bnd, what))
+    WORST.note("combine restatement vs fp64", R.check_bound(want, ref, bnd, what))
 
 
 @pytest.mark.parametrize("K", [1, 2, 3, 4, 5, 6, 7, 8, 16])
@@ -175,11 +113,11 @@ def test_combine_past_2g_elements():
     p = torch.rand((T, K), generator=g, device="cuda")
     res = torch.randn((T, H), generator=g, device="cuda").to(torch.bfloat16)
     out = torch.empty((T, H), dtype=torch.bfloat16, device="cuda")
-    _ok(combine(y, rmap, p, res, 0.7, T, K, H, out), "combine")
+    check(combine(y, rmap, p, res, 0.7, T, K, H, out), "combine")
     gout = torch.randn((T, H), generator=g, device="cuda").to(torch.bfloat16)
     act = torch.empty((M, H), dtype=torch.bfloat16, device="cuda")
     pg = torch.empty((T, K), dtype=torch.float32, device="cuda")
-    _ok(unpermute_bwd(gout, y, rmap, p, T, K, H, act, pg), "unpermute_bwd")
+    check(unpermute_bwd(gout, y, rmap, p, T, K, H, act, pg), "unpermute_bwd")
     torch.cuda.synchronize()
     far = (rmap.view(T, K).long() >= 2 ** 31 // H).any(1).nonzero().flatten()
     assert far.numel() > 0
@@ -193,22 +131,22 @@ def test_combine_past_2g_elements():
     want, _ = R.act_grad(gout[toks], local, p[toks], K, rows.numel())
     R.assert_bits_equal(act[rows], want, "act_grad past 2^31 elements")
     ref, bnd = R.prob_grad_ref(gout[toks], ys, local, K)
-    _note("prob_grad", R.check_bound(pg[toks], ref, bnd, "prob_grad past 2^31 elements"))
+    WORST.note("prob_grad", R.check_bound(pg[toks], ref, bnd, "prob_grad past 2^31 elements"))
     WORST["peak GiB, 2^31-element case"] = torch.cuda.max_memory_allocated() / 2 ** 30
     del y, act, out, gout, res, ys
     torch.cuda.empty_cache()
 
 
 def test_combine_refusals_name_the_entry():
-    lib = _lib()
+    lib = ensure_init()
     y = torch.zeros((8, 16), dtype=torch.bfloat16, device="cuda")
     m = torch.zeros(8, dtype=torch.int32, device="cuda")
     out = torch.empty((8, 16), dtype=torch.bfloat16, device="cuda")
-    assert lib.xtb_moe_combine(_p(y), _p(m), None, None, 1.0, 8, 1, 12, _p(out), _st()) == XTB_ERR_INVALID
+    assert lib.xtb_moe_combine(ptr(y), ptr(m), None, None, 1.0, 8, 1, 12, ptr(out), current_stream()) == XTB_ERR_INVALID
     assert b"xtb_moe_combine" in lib.xtb_last_error()
-    assert lib.xtb_moe_combine(_p(y), None, None, None, 1.0, 8, 1, 16, _p(out), _st()) == XTB_ERR_INVALID
+    assert lib.xtb_moe_combine(ptr(y), None, None, None, 1.0, 8, 1, 16, ptr(out), current_stream()) == XTB_ERR_INVALID
     assert b"xtb_moe_combine" in lib.xtb_last_error()
-    assert lib.xtb_moe_unpermute(_p(y), _p(m), None, 8, 1, 12, _p(out), _st()) == XTB_ERR_INVALID
+    assert lib.xtb_moe_unpermute(ptr(y), ptr(m), None, 8, 1, 12, ptr(out), current_stream()) == XTB_ERR_INVALID
     msg = lib.xtb_last_error()
     assert b"xtb_moe_unpermute" in msg and b"xtb_moe_combine" not in msg
 
@@ -229,22 +167,21 @@ def test_unpermute_bwd(K):
         p = R.probs(T, K, mode, seed + 3, "cuda") if i % 3 != 1 else None
         g = R.token_rows(R.token_scales(T, seed + 4, "cuda"), H, mode, seed + 5)
         M = T * K
-        abuf, act = _guarded(M, H)
-        pbuf, pg = _guarded(T, K, fp32=True)
-        _ok(unpermute_bwd(g, y, rmap, p, T, K, H, act, pg), what)
-        abuf2, act2 = _guarded(M, H)
-        _ok(unpermute_bwd(g, None, rmap, p, T, K, H, act2, None), what + " without prob_grad")
+        act, pg = Guarded(M, H, torch.bfloat16), Guarded(T, K, torch.float32)
+        check(unpermute_bwd(g, y, rmap, p, T, K, H, act.v, pg.v), what)
+        act2 = Guarded(M, H, torch.bfloat16)
+        check(unpermute_bwd(g, None, rmap, p, T, K, H, act2.v, None), what + " without prob_grad")
         torch.cuda.synchronize()
         want, written = R.act_grad(g, rmap, p, K, M)
-        _assert_guarded(abuf, M, what, written)
-        _assert_guarded(abuf2, M, what + " without prob_grad", written)
-        _assert_guarded(pbuf, T, what + " prob_grad")
-        R.assert_bits_equal(act[written], want[written], what)
-        assert torch.equal(abuf, abuf2), f"{what}: act_grad depends on whether prob_grad is asked for"
+        act.check(what, written)
+        act2.check(what + " without prob_grad", written)
+        pg.check(what + " prob_grad")
+        R.assert_bits_equal(act.v[written], want[written], what)
+        assert torch.equal(act.buf, act2.buf), f"{what}: act_grad depends on whether prob_grad is asked for"
         ref, bnd = R.prob_grad_ref(g, y, rmap, K)
-        _note("prob_grad", R.check_bound(pg, ref, bnd, what))
+        WORST.note("prob_grad", R.check_bound(pg.v, ref, bnd, what))
         neg = rmap.view(T, K) < 0
-        assert bool((pg[neg] == 0).all()), f"{what}: prob_grad of a -1 entry is not 0"
+        assert bool((pg.v[neg] == 0).all()), f"{what}: prob_grad of a -1 entry is not 0"
 
 
 # ---- rmsnorm (+ gate) --------------------------------------------------------------------------------------------------
@@ -256,29 +193,25 @@ def _norm_case(H, T, E, seed):
     gate_w = (torch.randn((E, H), generator=torch.Generator(device="cuda").manual_seed(seed + 2), device="cuda") * H ** -0.5
               if E else None)
     what = f"rmsnorm_gate H={H} T={T} E={E}"
-    xbuf, x = _guarded(T, H)
-    rbuf, rstd = _guarded(T, 1, fp32=True)
-    lbuf, logits = _guarded(T, max(E, 1), fp32=True)
-    _ok(rmsnorm_gate(h, w, gate_w, T, H, E, x, rstd, logits if E else None), what)
-    xbuf2, x2 = _guarded(T, H)
-    lbuf2, logits2 = _guarded(T, max(E, 1), fp32=True)
-    _ok(rmsnorm_gate(h, w, gate_w, T, H, E, x2, None, logits2 if E else None), what + " without rstd")
+    xg, rg, lg = Guarded(T, H, torch.bfloat16), Guarded(T, 1, torch.float32), Guarded(T, max(E, 1), torch.float32)
+    check(rmsnorm_gate(h, w, gate_w, T, H, E, xg.v, rg.v, lg.v if E else None), what)
+    xg2, lg2 = Guarded(T, H, torch.bfloat16), Guarded(T, max(E, 1), torch.float32)
+    check(rmsnorm_gate(h, w, gate_w, T, H, E, xg2.v, None, lg2.v if E else None), what + " without rstd")
     torch.cuda.synchronize()
-    _assert_guarded(xbuf, T, what + " x")
-    _assert_guarded(rbuf, T, what + " rstd")
+    x = xg.check(what + " x")
+    rs = rg.check(what + " rstd")[:, 0]
     if E:
-        _assert_guarded(lbuf, T, what + " logits")
-        assert torch.equal(lbuf, lbuf2), f"{what}: logits depend on whether rstd is written"
-    assert torch.equal(xbuf, xbuf2), f"{what}: x depends on whether rstd is written"
-    rs = rstd[:, 0]
+        lg.check(what + " logits")
+        assert torch.equal(lg.buf, lg2.buf), f"{what}: logits depend on whether rstd is written"
+    assert torch.equal(xg.buf, xg2.buf), f"{what}: x depends on whether rstd is written"
     ref = R.rstd_ref(h, R.EPS)
-    _note("rstd", R.check_bound(rs, ref, R.rstd_rel(H) * ref, what + " rstd"))
+    WORST.note("rstd", R.check_bound(rs, ref, R.rstd_rel(H) * ref, what + " rstd"))
     R.assert_bits_equal(x, R.rmsnorm_x(h, rs, w), what + " x given the kernel's rstd")
     xr, xb = R.x_ref(h, R.EPS, w)
-    _note("x (bf16, past the midpoint)", R.check_near_tie(x, xr, xb, what + " x"))
+    WORST.note("x (bf16, past the midpoint)", R.check_near_tie(x, xr, xb, what + " x")[0])
     if E:
         lr, lb = R.logits_ref(x, gate_w)
-        _note("gate logits", R.check_bound(logits, lr, lb, what + " logits"))
+        WORST.note("gate logits", R.check_bound(lg.v, lr, lb, what + " logits"))
 
 
 @pytest.mark.parametrize("H", [256, 512, 1024, 2048])
@@ -291,7 +224,7 @@ def test_rmsnorm(H):
 
 
 def test_rmsnorm_refusals():
-    lib = _lib()
+    lib = ensure_init()
     T = 4
     h = torch.zeros((T, 4096), dtype=torch.bfloat16, device="cuda")
     w = torch.ones(4096, dtype=torch.float32, device="cuda")
@@ -328,31 +261,32 @@ def _bwd_inputs(T, K, H, seed, mode="exact", rmap=None, owner=None):
 def _bwd_run(T, K, H, rmap, g_xp, gate, h, rstd, w, g_res, with_nw, what):
     """Runs without and with g_res; checks guards, the residual composition and that g_norm_w ignores g_res.
     Returns (g_h without g_res, g_norm_w or None)."""
-    hb0, gh0 = _guarded(T, H)
-    hb1, gh1 = _guarded(T, H)
-    nb0, nw0 = _guarded(1, H, fp32=True)
-    nb1, nw1 = _guarded(1, H, fp32=True)
-    _ok(dispatch_bwd(g_xp, rmap, gate, h, rstd, w, None, T, K, H, gh0, nw0[0] if with_nw else None), what)
-    _ok(dispatch_bwd(g_xp, rmap, gate, h, rstd, w, g_res, T, K, H, gh1, nw1[0] if with_nw else None), what + " +g_res")
+    gh0, gh1 = Guarded(T, H, torch.bfloat16), Guarded(T, H, torch.bfloat16)
+    nw0, nw1 = Guarded(1, H, torch.float32), Guarded(1, H, torch.float32)
+    check(dispatch_bwd(g_xp, rmap, gate, h, rstd, w, None, T, K, H, gh0.v, nw0.v[0] if with_nw else None), what)
+    check(dispatch_bwd(g_xp, rmap, gate, h, rstd, w, g_res, T, K, H, gh1.v, nw1.v[0] if with_nw else None),
+          what + " +g_res")
     torch.cuda.synchronize()
-    _assert_guarded(hb0, T, what + " g_h")
-    _assert_guarded(hb1, T, what + " g_h +g_res")
-    R.assert_bits_equal(gh1, (gh0.float() + g_res.float()).to(torch.bfloat16), what + " g_h(res) vs bf16(g_h + g_res)")
+    gh0.check(what + " g_h")
+    gh1.check(what + " g_h +g_res")
+    R.assert_bits_equal(gh1.v, (gh0.v.float() + g_res.float()).to(torch.bfloat16),
+                        what + " g_h(res) vs bf16(g_h + g_res)")
     if not with_nw:
-        assert bool((nb0 == FILL32).all() and (nb1 == FILL32).all()), f"{what}: g_norm_w written though NULL"
-        return gh0, None
-    _assert_guarded(nb0, 1, what + " g_norm_w")
-    assert torch.equal(nb0, nb1), f"{what}: g_norm_w depends on g_res"
-    return gh0, nw0[0]
+        nw0.check(what + " g_norm_w, NULL", written=False)
+        nw1.check(what + " g_norm_w, NULL +g_res", written=False)
+        return gh0.v, None
+    nw0.check(what + " g_norm_w")
+    assert torch.equal(nw0.buf, nw1.buf), f"{what}: g_norm_w depends on g_res"
+    return gh0.v, nw0.v[0]
 
 
 def _check_bwd(T, K, H, rmap, g_xp, gate, h, rstd, w, gh, nw, what):
     g_x = R.dispatch_gx(g_xp, rmap, gate, K)
     ref, bnd = R.g_h_ref(g_x, h, rstd, w)
-    _note("g_h (bf16, past the midpoint)", R.check_near_tie(gh, ref, bnd, what + " g_h"))
+    WORST.note("g_h (bf16, past the midpoint)", R.check_near_tie(gh, ref, bnd, what + " g_h")[0])
     if nw is not None:
         gr, gb = R.g_norm_w_ref(g_x, h, rstd, _n_cta(T))
-        _note("g_norm_w", R.check_bound(nw, gr, gb, what + " g_norm_w"))
+        WORST.note("g_norm_w", R.check_bound(nw, gr, gb, what + " g_norm_w"))
 
 
 @pytest.mark.parametrize("K", [1, 2, 3, 4, 6, 8])
@@ -460,7 +394,7 @@ def test_dispatch_bwd_refuses_wide_rows():
     w = torch.ones(H, device="cuda")
     out = torch.empty((T, H), dtype=torch.bfloat16, device="cuda")
     assert dispatch_bwd(z, m, None, z, r, w, None, T, 2, H, out, None) == XTB_ERR_INVALID
-    assert b"xtb_moe_dispatch_bwd_rmsnorm" in _lib().xtb_last_error()
+    assert b"xtb_moe_dispatch_bwd_rmsnorm" in ensure_init().xtb_last_error()
 
 
 def test_empty_batch_writes_nothing():
@@ -468,16 +402,17 @@ def test_empty_batch_writes_nothing():
     z = torch.zeros((4, H), dtype=torch.bfloat16, device="cuda")
     m = torch.zeros(4, dtype=torch.int32, device="cuda")
     f = torch.ones(H, device="cuda")
-    buf, out = _guarded(1, H)  # one row, so that the pointers are not NULL
-    fbuf, fout = _guarded(1, 1, fp32=True)
-    nb, nw = _guarded(1, H, fp32=True)
+    # one row each, so that the pointers are not NULL
+    out, fout, nw = Guarded(1, H, torch.bfloat16), Guarded(1, 1, torch.float32), Guarded(1, H, torch.float32)
     ws = torch.empty(1 << 20, dtype=torch.uint8, device="cuda")
-    lib = _lib()
-    assert lib.xtb_moe_combine(_p(z), _p(m), None, _p(z), 0.7, 0, K, H, _p(out), _st()) == 0
-    assert lib.xtb_moe_unpermute_bwd(_p(z), _p(z), _p(m), None, 0, K, H, _p(out), _p(fout), _st()) == 0
-    assert rmsnorm_gate(z, f, None, 0, H, 0, out, fout, None) == 0
-    assert lib.xtb_moe_dispatch_bwd_rmsnorm(_p(z), _p(m), None, _p(z), _p(f), _p(f), None, 0, K, H, _p(out), _p(nw[0]),
-                                            _p(ws), _st()) == 0
+    lib = ensure_init()
+    assert lib.xtb_moe_combine(ptr(z), ptr(m), None, ptr(z), 0.7, 0, K, H, ptr(out.v), current_stream()) == 0
+    assert lib.xtb_moe_unpermute_bwd(ptr(z), ptr(z), ptr(m), None, 0, K, H, ptr(out.v), ptr(fout.v),
+                                     current_stream()) == 0
+    assert rmsnorm_gate(z, f, None, 0, H, 0, out.v, fout.v, None) == 0
+    assert lib.xtb_moe_dispatch_bwd_rmsnorm(ptr(z), ptr(m), None, ptr(z), ptr(f), ptr(f), None, 0, K, H, ptr(out.v),
+                                            ptr(nw.v[0]), ptr(ws), current_stream()) == 0
     torch.cuda.synchronize()
-    assert bool((buf == FILL16).all() and (fbuf == FILL32).all() and (nb == FILL32).all()), "T = 0 wrote something"
-    assert math.isnan(float(nw[0, 0]))
+    for g, name in ((out, "bf16 out"), (fout, "fp32 out"), (nw, "g_norm_w")):
+        g.check(f"T = 0 wrote {name}", written=False)
+    assert math.isnan(float(nw.v[0, 0]))

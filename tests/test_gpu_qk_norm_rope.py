@@ -16,6 +16,7 @@ import pytest
 import torch
 
 from tests import qk_norm_rope_reference as R
+from tests.gpu_harness import sm_count
 from tests.norm_combine_reference import assert_bits_equal, check_bound, check_near_tie, norm_rows, norm_weight, rstd_rel
 
 pytestmark = pytest.mark.gpu
@@ -82,7 +83,7 @@ def test_forward_and_backward_against_the_references(T, Hq, Hkv, D, norm, gate):
     gq, gk = g_full[..., :D], torch.randn((T, Hkv, D), generator=g, device=DEV).to(torch.bfloat16)
     dx_q, dx_k, dw = _bwd(gq, gk, q, k, cos, sin, wq, wk, rq, rk)
     torch.cuda.synchronize()
-    n_cta = R.bwd_ctas(T, torch.cuda.get_device_properties(DEV).multi_processor_count)
+    n_cta = R.bwd_ctas(T, sm_count())
     worst = {}
     for i, (x, out, rstd, w, gg, dx) in enumerate(((q, out_q, rq, wq, gq, dx_q), (k, out_k, rk, wk, gk, dx_k))):
         tag = "qk"[i]

@@ -17,36 +17,15 @@ import pytest
 import torch
 
 from tests.router_reference import check_bound
+from xtuner_b200._capi import check, current_stream, ensure_init, ptr
 
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda"
 
 
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi.ensure_init()
-
-
-def _st():
-    from xtuner_b200._capi import current_stream
-
-    return current_stream()
-
-
-def _p(t):
-    return None if t is None else t.data_ptr()
-
-
-def _check(rc, what):
-    from xtuner_b200._capi import check
-
-    check(rc, what)
-
-
 def _ws(T, K, E):
-    return torch.zeros(int(_lib().xtb_moe_permute_workspace_bytes(T, K, E)), dtype=torch.uint8, device=DEV)
+    return torch.zeros(int(ensure_init().xtb_moe_permute_workspace_bytes(T, K, E)), dtype=torch.uint8, device=DEV)
 
 
 def _outs(T, E, K):
@@ -61,12 +40,14 @@ def greedy_route(logits, K, scoring, norm, scaling, ws=None):
     T, E = logits.shape
     o = _outs(T, E, K)
     if ws is None:
-        rc = _lib().xtb_router_greedy(_p(logits), T, E, K, scoring, int(norm), float(scaling), _p(o["rw"]), _p(o["tw"]),
-                                      _p(o["ids"]), _p(o["ids32"]), _p(o["tpe"]), _st())
+        rc = ensure_init().xtb_router_greedy(ptr(logits), T, E, K, scoring, int(norm), float(scaling), ptr(o["rw"]),
+                                             ptr(o["tw"]), ptr(o["ids"]), ptr(o["ids32"]), ptr(o["tpe"]),
+                                             current_stream())
     else:
-        rc = _lib().xtb_router_greedy_dispatch(_p(logits), T, E, K, scoring, int(norm), float(scaling), _p(o["rw"]),
-                                               _p(o["tw"]), _p(o["ids"]), _p(o["ids32"]), _p(o["tpe"]), _p(ws), _st())
-    _check(rc, "route")
+        rc = ensure_init().xtb_router_greedy_dispatch(ptr(logits), T, E, K, scoring, int(norm), float(scaling),
+                                                      ptr(o["rw"]), ptr(o["tw"]), ptr(o["ids"]), ptr(o["ids32"]),
+                                                      ptr(o["tpe"]), ptr(ws), current_stream())
+    check(rc, "route")
     return o
 
 
@@ -75,9 +56,9 @@ def greedy_replay(logits, replay, scoring, norm, scaling, ws=None):
     K = replay.shape[1]
     o = _outs(T, E, K)
     stride = replay.stride(0) if T else K
-    _check(_lib().xtb_router_greedy_replay(_p(logits), _p(replay), stride, T, E, K, scoring, int(norm), float(scaling),
-                                           _p(o["rw"]), _p(o["tw"]), _p(o["ids"]), _p(o["ids32"]), _p(o["tpe"]), _p(ws),
-                                           _st()), "replay")
+    check(ensure_init().xtb_router_greedy_replay(ptr(logits), ptr(replay), stride, T, E, K, scoring, int(norm),
+                                                 float(scaling), ptr(o["rw"]), ptr(o["tw"]), ptr(o["ids"]),
+                                                 ptr(o["ids32"]), ptr(o["tpe"]), ptr(ws), current_stream()), "replay")
     return o
 
 
@@ -148,8 +129,6 @@ def test_greedy_replay_of_own_ids_is_the_routing_bit_for_bit(E, scoring, norm, s
 @pytest.mark.parametrize("E,K", [(8, 2), (128, 8), (512, 8), (16, 1)])
 @pytest.mark.parametrize("scoring,norm", [(0, True), (1, False), (1, True)])
 def test_greedy_replay_random_ids_against_float64(E, K, scoring, norm):
-    from xtuner_b200 import _capi
-
     g = torch.Generator().manual_seed(7 * E + K)
     T, scaling = 333, 1.7
     logits = (torch.randn(T, E, generator=g) * 3).to(DEV)
@@ -168,8 +147,9 @@ def test_greedy_replay_random_ids_against_float64(E, K, scoring, norm):
     g_tw = torch.randn(T, K, generator=g).to(DEV)
     g_rw = torch.randn(T, E, generator=g).to(DEV)
     gl = torch.empty(T, E, device=DEV)
-    _capi.check(_lib().xtb_router_greedy_bwd(_p(o["rw"]), _p(o["tw"]), _p(o["ids"]), _p(g_tw), _p(g_rw), None, T, E, K,
-                                             scoring, int(norm), float(scaling), _p(gl), _st()), "bwd")
+    check(ensure_init().xtb_router_greedy_bwd(ptr(o["rw"]), ptr(o["tw"]), ptr(o["ids"]), ptr(g_tw), ptr(g_rw), None, T,
+                                              E, K, scoring, int(norm), float(scaling), ptr(gl), current_stream()),
+          "bwd")
     lg = logits.cpu().double().requires_grad_(True)
     p = torch.softmax(lg, 1) if scoring == 0 else torch.sigmoid(lg)
     w = p.gather(1, ids.cpu())
@@ -218,13 +198,15 @@ def test_out_of_range_ids_give_nan_weights_for_that_token_only_and_stay_in_bound
     assert torch.equal(o["ids"], fixed)
     assert torch.equal(o["tpe"].cpu(), torch.bincount(fixed.flatten().cpu(), minlength=E))
     # permute + combine over those outputs: in bounds, NaN rows only for the bad tokens
-    lib = _lib()
+    lib = ensure_init()
     x = torch.randn(T, H, generator=g).to(torch.bfloat16).to(DEV)
     xp = torch.empty(T * K, H, dtype=torch.bfloat16, device=DEV)
     rmap = torch.empty(T * K, dtype=torch.int32, device=DEV)
-    _check(lib.xtb_moe_permute_prepared(_p(x), _p(o["ids32"]), T, K, E, H * 2, _p(xp), _p(rmap), None, _p(ws), _st()), "permute")
+    check(lib.xtb_moe_permute_prepared(ptr(x), ptr(o["ids32"]), T, K, E, H * 2, ptr(xp), ptr(rmap), None, ptr(ws),
+                                       current_stream()), "permute")
     out = torch.empty(T, H, dtype=torch.bfloat16, device=DEV)
-    _check(lib.xtb_moe_combine(_p(xp), _p(rmap), _p(o["tw"]), None, 1.0, T, K, H, _p(out), _st()), "combine")
+    check(lib.xtb_moe_combine(ptr(xp), ptr(rmap), ptr(o["tw"]), None, 1.0, T, K, H, ptr(out), current_stream()),
+          "combine")
     torch.cuda.synchronize()
     assert torch.isnan(out[rows].float()).all()
     assert torch.isfinite(out[keep.to(DEV)].float()).all()
@@ -252,14 +234,15 @@ def _gate_route(x, w, K_or_ids, scoring, norm, scaling, ws, replay=False):
     o = _outs(T, E, K)
     o["logits"] = torch.full((T, E), float("nan"), device=DEV)
     if replay:
-        rc = _lib().xtb_gate_route_replay_dispatch(_p(x), _p(w), _p(K_or_ids), K_or_ids.stride(0) if T else K, T, H, E, K,
-                                                   scoring, int(norm), float(scaling), _p(o["logits"]), _p(o["rw"]),
-                                                   _p(o["tw"]), _p(o["ids"]), _p(o["ids32"]), _p(o["tpe"]), _p(ws), _st())
+        rc = ensure_init().xtb_gate_route_replay_dispatch(ptr(x), ptr(w), ptr(K_or_ids), K_or_ids.stride(0) if T else K,
+                                                          T, H, E, K, scoring, int(norm), float(scaling),
+                                                          ptr(o["logits"]), ptr(o["rw"]), ptr(o["tw"]), ptr(o["ids"]),
+                                                          ptr(o["ids32"]), ptr(o["tpe"]), ptr(ws), current_stream())
     else:
-        rc = _lib().xtb_gate_route_dispatch(_p(x), _p(w), T, H, E, K, scoring, int(norm), float(scaling), _p(o["logits"]),
-                                            _p(o["rw"]), _p(o["tw"]), _p(o["ids"]), _p(o["ids32"]), _p(o["tpe"]), _p(ws),
-                                            _st())
-    _check(rc, "gate_route")
+        rc = ensure_init().xtb_gate_route_dispatch(ptr(x), ptr(w), T, H, E, K, scoring, int(norm), float(scaling),
+                                                   ptr(o["logits"]), ptr(o["rw"]), ptr(o["tw"]), ptr(o["ids"]),
+                                                   ptr(o["ids32"]), ptr(o["tpe"]), ptr(ws), current_stream())
+    check(rc, "gate_route")
     return o
 
 
@@ -289,8 +272,9 @@ def noaux_route(logits, bias, K, n_group, topk_group, norm, scaling):
     T, E = logits.shape
     o = _outs(T, E, K)
     o["tpe"] = torch.full((E,), -7.0, device=DEV)
-    _check(_lib().xtb_router_noaux(_p(logits), _p(bias), T, E, K, n_group, topk_group, int(norm), float(scaling), _p(o["rw"]),
-                                   _p(o["tw"]), _p(o["ids"]), _p(o["ids32"]), _p(o["tpe"]), _st()), "noaux")
+    check(ensure_init().xtb_router_noaux(ptr(logits), ptr(bias), T, E, K, n_group, topk_group, int(norm),
+                                         float(scaling), ptr(o["rw"]), ptr(o["tw"]), ptr(o["ids"]), ptr(o["ids32"]),
+                                         ptr(o["tpe"]), current_stream()), "noaux")
     return o
 
 
@@ -299,15 +283,15 @@ def noaux_replay(logits, bias, replay, n_group, topk_group, norm, scaling):
     K = replay.shape[1]
     o = _outs(T, E, K)
     o["tpe"] = torch.full((E,), -7.0, device=DEV)
-    _check(_lib().xtb_router_noaux_replay(_p(logits), _p(bias), _p(replay), replay.stride(0) if T else K, T, E, K, n_group,
-                                          topk_group, int(norm), float(scaling), _p(o["rw"]), _p(o["tw"]), _p(o["ids"]),
-                                          _p(o["ids32"]), _p(o["tpe"]), _st()), "noaux_replay")
+    check(ensure_init().xtb_router_noaux_replay(ptr(logits), ptr(bias), ptr(replay), replay.stride(0) if T else K, T, E,
+                                                K, n_group, topk_group, int(norm), float(scaling), ptr(o["rw"]),
+                                                ptr(o["tw"]), ptr(o["ids"]), ptr(o["ids32"]), ptr(o["tpe"]),
+                                                current_stream()), "noaux_replay")
     return o
 
 
 @pytest.mark.parametrize("E,K,n_group,topk_group", [(256, 8, 8, 4), (256, 8, 8, 8), (64, 6, 4, 2), (512, 8, 16, 16)])
 def test_noaux_replay_own_ids_bit_for_bit_and_random_ids_against_float64(E, K, n_group, topk_group):
-    from xtuner_b200 import _capi
     from xtuner_b200.router import noaux_group_spec
 
     g = torch.Generator().manual_seed(E + K + n_group)
@@ -327,9 +311,9 @@ def test_noaux_replay_own_ids_bit_for_bit_and_random_ids_against_float64(E, K, n
         g_tw = torch.randn(T, K, generator=g).to(DEV)
         g_rw = torch.randn(T, E, generator=g).to(DEV)
         gl = torch.empty(T, E, device=DEV)
-        _capi.check(_lib().xtb_router_noaux_bwd(_p(logits), _p(bias), _p(o["rw"]), _p(o["tw"]), _p(o["ids"]), _p(g_tw),
-                                                _p(g_rw), T, E, K, noaux_group_spec(n_group, topk_group), 1, 2.5, _p(gl),
-                                                _st()), "noaux_bwd")
+        check(ensure_init().xtb_router_noaux_bwd(ptr(logits), ptr(bias), ptr(o["rw"]), ptr(o["tw"]), ptr(o["ids"]),
+                                                 ptr(g_tw), ptr(g_rw), T, E, K, noaux_group_spec(n_group, topk_group),
+                                                 1, 2.5, ptr(gl), current_stream()), "noaux_bwd")
         lg = logits.cpu().double().requires_grad_(True)
         r, w = noaux_replay_ref(lg, bias.cpu(), ids.cpu(), K, n_group, topk_group, True, 2.5)
         (w * g_tw.cpu().double()).sum().add((r * g_rw.cpu().double()).sum()).backward()

@@ -15,63 +15,30 @@ import pytest
 import torch
 
 from tests import swiglu_fp8_reference as R
+from tests.gpu_harness import Guarded
+from xtuner_b200._capi import check, current_stream, ensure_init
 
 pytestmark = pytest.mark.gpu
-
-GUARD = 16
-FILL = 0x7FA5  # a bf16 NaN no kernel produces
-
-
-def _lib():
-    from xtuner_b200 import _capi
-
-    return _capi.ensure_init()
-
-
-def _st():
-    from xtuner_b200._capi import current_stream
-
-    return current_stream()
-
-
-def _ok(rc, what):
-    from xtuner_b200._capi import check
-
-    check(rc, what)
-
-
-def _guarded(rows, cols):
-    buf = torch.full((rows + 2 * GUARD, cols), FILL, dtype=torch.int16, device="cuda")
-    return buf, buf[GUARD : GUARD + rows].view(torch.bfloat16)
-
-
-def _assert_guarded(buf, rows, what):
-    assert bool((buf[:GUARD] == FILL).all() and (buf[GUARD + rows :] == FILL).all()), f"{what}: a guard row was written"
-    if rows:
-        unwritten = buf[GUARD : GUARD + rows] == FILL
-        assert not bool(unwritten.any()), f"{what}: {int(unwritten.sum())} output elements never written"
 
 
 def fwd(h, out):
     M, twoI = h.shape
-    _ok(_lib().xtb_swiglu(h.data_ptr(), out.data_ptr(), M, twoI // 2, _st()), "xtb_swiglu")
+    check(ensure_init().xtb_swiglu(h.data_ptr(), out.data_ptr(), M, twoI // 2, current_stream()), "xtb_swiglu")
 
 
 def bwd(d, h, gh):
     M, twoI = h.shape
-    _ok(_lib().xtb_swiglu_bwd(d.data_ptr(), h.data_ptr(), gh.data_ptr(), M, twoI // 2, _st()), "xtb_swiglu_bwd")
+    check(ensure_init().xtb_swiglu_bwd(d.data_ptr(), h.data_ptr(), gh.data_ptr(), M, twoI // 2, current_stream()),
+          "xtb_swiglu_bwd")
 
 
 def _run(h, d):
     M, twoI = h.shape
-    abuf, a = _guarded(M, twoI // 2)
-    gbuf, gh = _guarded(M, twoI)
-    fwd(h, a)
-    bwd(d, h, gh)
+    a, gh = Guarded(M, twoI // 2, torch.bfloat16), Guarded(M, twoI, torch.bfloat16)
+    fwd(h, a.v)
+    bwd(d, h, gh.v)
     torch.cuda.synchronize()
-    _assert_guarded(abuf, M, "swiglu")
-    _assert_guarded(gbuf, M, "swiglu_bwd")
-    return a, gh
+    return a.check("swiglu"), gh.check("swiglu_bwd")
 
 
 def test_swiglu_every_bf16_gate_value():
@@ -123,9 +90,7 @@ def test_swiglu_shapes_in_guard_bands(M, I):
 def test_swiglu_bwd_right_behind_the_grouped_gemm():
     """g_a from xtb_group_gemm_nn with xtb_swiglu_bwd launched straight after it on the same stream (fused.py), as a
     programmatic dependent launch: the result equals the same backward on a synchronised copy of g_a."""
-    from xtuner_b200._capi import check
-
-    lib = _lib()
+    lib = ensure_init()
     gen = torch.Generator("cuda").manual_seed(11)
     E, H = 8, 512
     for I in (768, 1536):
@@ -136,7 +101,7 @@ def test_swiglu_bwd_right_behind_the_grouped_gemm():
         h = (torch.randn(M, 2 * I, generator=gen, device="cuda") * 2).to(torch.bfloat16)
         g_a = torch.empty(M, I, dtype=torch.bfloat16, device="cuda")
         g_h = torch.empty(M, 2 * I, dtype=torch.bfloat16, device="cuda")
-        st = _st()
+        st = current_stream()
         check(lib.xtb_group_gemm_nn(g_y.data_ptr(), w2.data_ptr(), tpe.data_ptr(), M, H, I, E, g_a.data_ptr(), st),
               "xtb_group_gemm_nn")
         check(lib.xtb_swiglu_bwd(g_a.data_ptr(), h.data_ptr(), g_h.data_ptr(), M, I, st), "xtb_swiglu_bwd")
