@@ -361,6 +361,34 @@ int xtb_qk_norm_rope_bwd(const void* g_q_bf16, int64_t g_q_stride_t, int64_t g_q
                          const float* rstd_q, const float* rstd_k, int T, int Hq, int Hkv, int D, void* dx_q_bf16,
                          void* dx_k_bf16, float* dw, void* workspace, xtb_stream_t stream);
 
+/* MoE auxiliary-loss statistics of one layer (AuxLossContext.accumulate, loss/aux_loss.py:84-151, with
+ * BalancingLossContext.accumulate and ZLossContext.accumulate, loss/moe_loss.py:106-119,242-289), one kernel each way.
+ *   rw [N, E] fp32 router weights, logits [N, E] fp32 router logits, ids [N, K] int64 expert ids: the non-pad rows the
+ *   reference selects, contiguous.  1 <= E <= 512, K >= 1 (XTB_ERR_INVALID otherwise).  Row offsets are 64-bit.
+ * Forward, reading each input once:
+ *   tokens_per_expert [E] int64 = torch.histc(ids.float(), bins=E, min=0, max=E).long() exactly: id e in [0, E) counts in
+ *       bin e, id == E in bin E - 1; ids < 0 or > E are not counted.
+ *   rw_sum [E] fp32 = rw.sum(dim=0)                                      (NULL to skip; rw is then not read)
+ *   lse [N] fp32 = m + logf(sum_e expf(x_e - m)), m = max_e x_e, or 0 where that max is +-inf (torch.logsumexp's
+ *       masked_fill), accurate expf / logf: a NaN in the row gives NaN, an all -inf row gives -inf
+ *   z_sum 0-d fp32 = sum_t lse_t^2                                       (NULL to skip all z work: logits and lse are
+ *       then neither read nor written)
+ *   The sums are per-CTA partials added in a fixed order by the last CTA to finish, so two calls give the same bits.
+ *   N == 0 writes zero counts and sums (the inputs may then be NULL).  workspace: xtb_moe_aux_stats_workspace_bytes(N, E)
+ *   bytes whose first 4 bytes are zero before the first call; every call leaves them zero (no memset between calls).
+ *   Calls sharing a workspace must be ordered on one stream.
+ * Backward, one elementwise pass over the outputs asked for (N == 0, or both outputs NULL, is a no-op):
+ *   g_rw [N, E] fp32     = g_rw_sum[e]                        (the broadcast of sum's backward; NULL to skip)
+ *   g_logits [N, E] fp32 = (g_z (2 lse_t)) expf(x_te - lse_t)  (torch's pow and logsumexp backward order; NULL to skip)
+ *   g_rw_sum [E] and g_z (0-d) are device pointers, at least one of them given: nothing is read on the host.
+ * Neither entry allocates or synchronises the host, so both can be captured in a CUDA graph. */
+size_t xtb_moe_aux_stats_workspace_bytes(int64_t N, int E);
+int xtb_moe_aux_stats(const float* rw, const float* logits, const int64_t* ids, int64_t N, int E, int K,
+                      int64_t* tokens_per_expert, float* rw_sum, float* z_sum, float* lse, void* workspace,
+                      xtb_stream_t stream);
+int xtb_moe_aux_stats_bwd(const float* g_rw_sum, const float* g_z, const float* logits, const float* lse, int64_t N,
+                          int E, float* g_rw, float* g_logits, xtb_stream_t stream);
+
 /* ==== fp8 tile-wise quantisation (row a15, config 5) ============================================================
  * e4m3, scale = clamp(amax, 1e-12) / 448 (xtuner/v1/float8/float8_utils.py:6-32, fsdp_utils.py:75-116,195-223,
  * triton_kernels/per_tile_quant.py:61-100).  Bit-exact on an H100 against reference-made golden vectors

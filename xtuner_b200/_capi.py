@@ -119,7 +119,11 @@ SIGNATURES = {
          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
          c_void_p, c_void_p],
     ),
-    "xtb_fp8_per_tile_quant": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
+    "xtb_moe_aux_stats_workspace_bytes": (c_size_t, [c_int64, c_int]),
+    "xtb_moe_aux_stats": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "xtb_moe_aux_stats_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "xtb_fp8_per_tile_quant":(c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "xtb_fp8_block_scales": (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_void_p, c_void_p]),
     "xtb_fp8_block_cast": (c_int, [c_void_p, c_int, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "xtb_peer_barrier": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p]),

@@ -19,7 +19,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libxtuner_b200.so")
 OBJ_DIR = os.path.join(PKG_DIR, "build")
 
 SOURCES = ["lib.cu", "route.cu", "gate_mma.cu", "gate_route_replay.cu", "permute.cu", "group_gemm.cu", "comm.cu", "ep.cu", "norm.cu", "fp8.cu", "lm_head_ce.cu",
-           "qk_norm_rope.cu"]
+           "qk_norm_rope.cu", "moe_aux_loss.cu"]
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 

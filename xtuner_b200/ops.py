@@ -21,7 +21,7 @@ from . import _capi
 from ._capi import check, current_stream, ptr
 
 __all__ = ["permute", "unpermute", "group_gemm", "swiglu", "gate_logits", "permute_workspace", "lm_head_cross_entropy",
-           "lm_head_logprobs", "qk_norm_rope"]
+           "lm_head_logprobs", "qk_norm_rope", "moe_aux_stats"]
 
 
 def _require_cuda(*tensors: Tensor) -> None:
@@ -748,6 +748,103 @@ def qk_norm_rope(q: Tensor, k: Tensor, cos: Tensor, sin: Tensor, q_norm_weight: 
         w_q, w_k = q_norm_weight.float().contiguous(), k_norm_weight.float().contiguous()  # bf16 widens exactly
     out_q, out_k, _, _ = _QKNormRope.apply(q, k, cos.contiguous(), sin.contiguous(), w_q, w_k, float(eps))
     return out_q, out_k
+
+
+# ======================================================================================================
+# MoE auxiliary-loss statistics (AuxLossContext.accumulate, loss/aux_loss.py:84-151)
+# ======================================================================================================
+
+MOE_AUX_MAX_EXPERTS = 512  # the largest E xtb_moe_aux_stats takes
+
+
+def _moe_aux_workspace(N: int, E: int, device) -> Tensor:
+    """zero-filled once: the kernel's ticket must start at zero, and every call leaves it so"""
+    need = int(_capi.ensure_init().xtb_moe_aux_stats_workspace_bytes(N, E))
+    key = ("moe_aux", device, torch.cuda.current_stream(device).cuda_stream)
+    ws = _workspaces.get(key)
+    if ws is None or ws.numel() < need:
+        ws = torch.zeros(max(need, 1 << 16), dtype=torch.uint8, device=device)
+        _workspaces[key] = ws
+    return ws
+
+
+def _plain(t: Tensor) -> Tensor:
+    """the tensor behind a pending functional collective's result (``AsyncCollectiveTensor.wait()``), else ``t``"""
+    return t.wait() if type(t) is not Tensor and hasattr(t, "wait") else t
+
+
+class _MoEAuxStats(torch.autograd.Function):
+    """One node over ``xtb_moe_aux_stats`` / ``xtb_moe_aux_stats_bwd``.  Saves the logits and the row logsumexps only for
+    the z-loss; an output that receives no gradient gives its input no gradient (no zero ``[N, E]`` tensor is made)."""
+
+    @staticmethod
+    def forward(ctx, rw: Tensor, logits: Optional[Tensor], ids: Tensor, n_experts: int, need_rw_sum: bool, need_z: bool):
+        ctx.set_materialize_grads(False)
+        N, K = ids.shape
+        dev = ids.device
+        tpe = torch.empty((n_experts,), dtype=torch.int64, device=dev)
+        rw_sum = torch.empty((n_experts,), dtype=torch.float32, device=dev) if need_rw_sum else None
+        z_sum = torch.empty((), dtype=torch.float32, device=dev) if need_z else None
+        lse = torch.empty((N,), dtype=torch.float32, device=dev) if need_z else None
+        lib = _capi.ensure_init()
+        ws = _moe_aux_workspace(N, n_experts, dev)
+        check(lib.xtb_moe_aux_stats(ptr(rw) if need_rw_sum else None, ptr(logits) if need_z else None, ptr(ids), N,
+                                    n_experts, K, ptr(tpe), ptr(rw_sum), ptr(z_sum), ptr(lse), ptr(ws), current_stream()),
+              "xtb_moe_aux_stats")
+        ctx.mark_non_differentiable(tpe)
+        if need_z:
+            ctx.save_for_backward(logits, lse)
+        ctx.shape = (N, n_experts)
+        return tpe, rw_sum, z_sum
+
+    @staticmethod
+    def backward(ctx, _g_tpe, g_rw_sum, g_z):
+        N, E = ctx.shape
+        need_rw = g_rw_sum is not None and ctx.needs_input_grad[0]
+        need_lg = g_z is not None and ctx.needs_input_grad[1]
+        if not (need_rw or need_lg):
+            return None, None, None, None, None, None
+        logits, lse = ctx.saved_tensors if need_lg else (None, None)
+        dev = (g_rw_sum if need_rw else g_z).device
+        g_rw = torch.empty((N, E), dtype=torch.float32, device=dev) if need_rw else None
+        g_logits = torch.empty((N, E), dtype=torch.float32, device=dev) if need_lg else None
+        # held in locals until the launch is queued.  An expanded gradient becomes a contiguous copy; one that comes from a
+        # functional all-reduce (the global-average balancing loss) is an AsyncCollectiveTensor, whose data pointer is only
+        # valid after wait()
+        g_rw_sum = _plain(g_rw_sum).float().contiguous() if need_rw else None
+        g_z = _plain(g_z).float().contiguous() if need_lg else None
+        check(_capi.ensure_init().xtb_moe_aux_stats_bwd(ptr(g_rw_sum), ptr(g_z), ptr(logits), ptr(lse), N, E, ptr(g_rw),
+                                                        ptr(g_logits), current_stream()), "xtb_moe_aux_stats_bwd")
+        return g_rw, g_logits, None, None, None, None
+
+
+def moe_aux_stats(router_weights: Tensor, router_logits: Tensor | None, selected_experts: Tensor, n_experts: int, *,
+                  need_rw_sum: bool = True, need_z: bool = False):
+    """The statistics ``AuxLossContext.accumulate`` derives from one layer's router (loss/aux_loss.py:84-151), in one
+    kernel: ``(tokens_per_expert, rw_sum, z_sum)`` with
+
+    * ``tokens_per_expert`` int64 ``[E]`` = ``torch.histc(selected_experts.float(), bins=E, min=0, max=E).long()``,
+      exactly (ids equal to E count in the last bin, ids below 0 or above E nowhere); not differentiable;
+    * ``rw_sum`` fp32 ``[E]`` = ``router_weights.sum(dim=0)`` (None unless ``need_rw_sum``);
+    * ``z_sum`` 0-d fp32 = ``torch.logsumexp(router_logits, -1).square().sum()`` (None unless ``need_z``).
+
+    ``router_weights`` and ``router_logits`` are fp32 ``[N, E]``, ``selected_experts`` int64 ``[N, K]``, all CUDA;
+    ``1 <= E <=`` :data:`MOE_AUX_MAX_EXPERTS`.  Sums are added in a fixed order: the same inputs give the same bits."""
+    _require_cuda(router_weights, router_logits, selected_experts)
+    E = int(n_experts)
+    if not 1 <= E <= MOE_AUX_MAX_EXPERTS:
+        raise _capi.XtbError(f"moe_aux_stats: n_experts={E} is outside [1, {MOE_AUX_MAX_EXPERTS}]")
+    if selected_experts.dim() != 2 or selected_experts.dtype != torch.int64 or selected_experts.shape[1] < 1:
+        raise _capi.XtbError(f"moe_aux_stats: selected_experts must be int64 [N, K] (got {tuple(selected_experts.shape)} "
+                             f"{selected_experts.dtype})")
+    N = selected_experts.shape[0]
+    for t, name, need in ((router_weights, "router_weights", need_rw_sum), (router_logits, "router_logits", need_z)):
+        if need and (t is None or t.dtype != torch.float32 or tuple(t.shape) != (N, E)):
+            raise _capi.XtbError(f"moe_aux_stats: {name} must be float32 [{N}, {E}] (got "
+                                 f"{None if t is None else (tuple(t.shape), t.dtype)})")
+    rw = router_weights.contiguous() if need_rw_sum else router_weights
+    logits = router_logits.contiguous() if need_z else router_logits
+    return _MoEAuxStats.apply(rw, logits, selected_experts.contiguous(), E, bool(need_rw_sum), bool(need_z))
 
 
 # ======================================================================================================

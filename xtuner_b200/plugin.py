@@ -21,7 +21,8 @@ activation memory for the same results, without checkpointing the whole decoder 
 Everything else of the model (attention, norms, lm_head, FSDP wrapping, checkpoint keys) is untouched;
 ``install_lm_head_loss()`` separately moves the lm_head cross-entropy onto this package's kernels,
 ``install_rl_lm_head()`` the RL trainer's lm_head log-probabilities and GRPO loss, and
-``install_qk_norm_rope(model)`` the q/k norm and rotary embedding in front of the attention; parameters keep their
+``install_qk_norm_rope(model)`` the q/k norm and rotary embedding in front of the attention, and
+``install_moe_aux_loss()`` the statistics behind the MoE balancing and z losses; parameters keep their
 names, so state dicts and DCP checkpoints stay compatible.  ``restore_model`` undoes the conversion.
 """
 from __future__ import annotations
@@ -572,3 +573,80 @@ def uninstall_qk_norm_rope(model: nn.Module) -> None:
             del attn.q_norm.forward
             del attn.k_norm.forward
         delattr(attn, _QK_SAVED)
+
+
+# ======================================================================================================
+# MoE auxiliary losses: the statistics AuxLossContext.accumulate takes from every MoE layer's router
+# ======================================================================================================
+
+
+def _aux_eligible(aux, classes, bal, zs, rw, logits, ids) -> bool:
+    """what ``ops.moe_aux_stats`` computes: the reference's own context classes (a subclass may change what they do),
+    fp32 ``[N, E]`` weights and logits and int64 ``[N, K]`` ids on the device, ``E`` within the kernel's range"""
+    aux_cls, bal_cls, z_cls = classes
+    E = aux.n_routed_experts
+    return (type(aux) is aux_cls and all(type(c) is bal_cls for c in bal) and all(type(c) is z_cls for c in zs)
+            and 1 <= E <= ops.MOE_AUX_MAX_EXPERTS
+            and all(type(t) is torch.Tensor and _on_device(t) for t in (rw, logits, ids))
+            and ids.dtype == torch.int64 and ids.dim() == 2 and ids.shape[1] >= 1
+            and all(t.dtype == torch.float32 and tuple(t.shape) == (ids.shape[0], E) for t in (rw, logits)))
+
+
+def install_moe_aux_loss() -> None:
+    """Rebinds ``AuxLossContext.accumulate`` (``xtuner/v1/loss/aux_loss.py``) so that each MoE layer's expert counts, the
+    balancing contexts' router-weight sums and the z-loss sum of squared logsumexps come from one
+    :func:`ops.moe_aux_stats` call, forward and backward, instead of the reference's eager chain of ``histc``, ``sum``
+    and ``logsumexp``.  Everything around them is the reference's: the counts go to ``_local_load_logits_list``, the sum
+    to each balancing context's ``routing_weights_sum_list``, and each z context applies its own scaling (the alpha 0
+    branch, ``/ denom_local``, the global-average factor with the device tensor ``num_tokens_global``, ``* alpha /
+    batch_size``), updates its running log value and is attached to the hidden states through ``AuxLossScaler``.
+    ``finalize`` is untouched.  Calls it does not cover run the original method: context subclasses, non-CUDA tensors,
+    weights or logits that are not fp32 ``[N, E]``, ids that are not int64 ``[N, K]``, and ``E`` above
+    :data:`ops.MOE_AUX_MAX_EXPERTS`.  Opt-in; installing twice is harmless, and it composes with :func:`convert_model`
+    and the other installs."""
+    aux_mod = importlib.import_module("xtuner.v1.loss.aux_loss")
+    moe_loss = importlib.import_module("xtuner.v1.loss.moe_loss")
+    cls = aux_mod.AuxLossContext
+    if _SAVED in vars(cls):
+        return
+    orig = vars(cls)["accumulate"]
+    classes = (cls, moe_loss.BalancingLossContext, moe_loss.ZLossContext)
+
+    def accumulate(self, *, selected_router_weights, selected_router_logits, selected_experts, hidden_states,
+                   balancing_ctx=None, z_ctx=None, num_tokens_local=0, num_tokens_global=None, world_size=1):
+        bal, zs = aux_mod._as_list(balancing_ctx), aux_mod._as_list(z_ctx)
+        if not _aux_eligible(self, classes, bal, zs, selected_router_weights, selected_router_logits, selected_experts):
+            return orig(self, selected_router_weights=selected_router_weights,
+                        selected_router_logits=selected_router_logits, selected_experts=selected_experts,
+                        hidden_states=hidden_states, balancing_ctx=balancing_ctx, z_ctx=z_ctx,
+                        num_tokens_local=num_tokens_local, num_tokens_global=num_tokens_global, world_size=world_size)
+        tokens_per_expert, rw_sum, z_sum = ops.moe_aux_stats(
+            selected_router_weights, selected_router_logits, selected_experts, self.n_routed_experts,
+            need_rw_sum=bool(bal), need_z=any(ctx.loss_cfg.z_loss_alpha != 0 for ctx in zs))
+        self._local_load_logits_list.append(tokens_per_expert)
+        for ctx in bal:
+            ctx.routing_weights_sum_list.append(rw_sum)
+        for ctx in zs:
+            if ctx.loss_cfg.z_loss_alpha == 0:
+                loss = torch.tensor(0.0, device=selected_router_logits.device, dtype=torch.float32)
+                ctx._update_running(loss)
+            else:  # ZLossContext.accumulate's scaling lines, applied to the kernel's sum of lse^2
+                loss = z_sum / max(num_tokens_local, 1)
+                if ctx.loss_cfg.z_loss_global_average and num_tokens_global is not None:
+                    denom_global = torch.clamp(num_tokens_global, min=1)
+                    loss = loss * num_tokens_local * world_size / denom_global
+                loss = loss * ctx.loss_cfg.z_loss_alpha / ctx._batch_size
+                ctx._update_running(loss.detach())
+            hidden_states = aux_mod.AuxLossScaler.apply(hidden_states, loss)
+        return hidden_states
+
+    accumulate.__wrapped__ = orig
+    setattr(cls, _SAVED, orig)
+    cls.accumulate = accumulate
+
+
+def uninstall_moe_aux_loss() -> None:
+    cls = importlib.import_module("xtuner.v1.loss.aux_loss").AuxLossContext
+    if _SAVED in vars(cls):
+        cls.accumulate = vars(cls)[_SAVED]
+        delattr(cls, _SAVED)
