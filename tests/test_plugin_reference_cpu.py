@@ -410,7 +410,7 @@ def test_convert_model_leaves_unsupported_layers_whole_and_group_gemm_falls_back
         import importlib
 
         mgl = importlib.import_module("xtuner.v1.module.grouped_linear.moe_group_linear")
-        original = getattr(mgl, plugin._SAVED)
+        original = vars(mgl)[plugin._SAVED]["group_gemm"]
         x = torch.randn(6, 64).to(torch.bfloat16)  # CPU, width 64: not eligible -> the reference's own op answers
         w = torch.randn(2, 32, 64).to(torch.bfloat16)
         tpe = torch.tensor([2, 4])

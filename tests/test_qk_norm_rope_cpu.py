@@ -276,7 +276,7 @@ def test_plugin_skips_ineligible_layers(ref):
                                   _attn(ref, qk_norm=False)])
     assert plugin.install_qk_norm_rope(layers) == 2
     assert plugin.install_qk_norm_rope(layers) == 0  # installed layers are not wrapped twice
-    assert [plugin._QK_SAVED in vars(a) for a in layers] == [False, False, False, True, True]
+    assert [plugin._SAVED in vars(a) for a in layers] == [False, False, False, True, True]
     plugin.uninstall_qk_norm_rope(layers)
 
 

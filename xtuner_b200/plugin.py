@@ -27,9 +27,9 @@ names, so state dicts and DCP checkpoints stay compatible.  ``restore_model`` un
 """
 from __future__ import annotations
 
+import functools
 import importlib
 import types
-from typing import Any
 
 import torch
 from torch import nn
@@ -40,6 +40,36 @@ from .dispatcher import FusedDispatcher
 from .router import GreedyRouter, NoAuxRouter
 
 _SAVED = "_xtuner_b200_saved"
+_ABSENT = object()  # saved for a name the owner did not carry itself (a class attribute showed through)
+
+
+def _rebind(owner, **replacements) -> bool:
+    """Sets each name on ``owner`` (a class, a module or an object) and keeps what the owner itself held under it in
+    ``vars(owner)[_SAVED]``, for :func:`_restore`: a class's raw entry (descriptors such as ``staticmethod`` survive,
+    subclasses keep inheriting), an ``nn.Module``'s registered submodule, or :data:`_ABSENT`.  An owner that already
+    carries a rebind is left as it is and False returned: installing twice changes nothing."""
+    if _SAVED in vars(owner):
+        return False
+    subs = owner._modules if isinstance(owner, nn.Module) else {}
+    saved = {name: subs[name] if name in subs else vars(owner).get(name, _ABSENT) for name in replacements}
+    setattr(owner, _SAVED, saved)
+    for name, value in replacements.items():
+        setattr(owner, name, value)
+    return True
+
+
+def _restore(owner) -> None:
+    """Puts back what :func:`_rebind` saved on ``owner``: ``setattr`` (so a submodule is registered again), or deletes
+    the name the owner did not carry before.  Nothing to do when the owner carries no rebind."""
+    saved = vars(owner).get(_SAVED)
+    if saved is None:
+        return
+    for name, original in saved.items():
+        if original is _ABSENT:
+            delattr(owner, name)
+        else:
+            setattr(owner, name, original)
+    delattr(owner, _SAVED)
 
 
 def _router_convertible(router: nn.Module) -> bool:
@@ -106,9 +136,10 @@ def _fused_eligible(layer: nn.Module) -> bool:
     )
 
 
-def _fused_layer_forward(self, hidden_states, seq_ctx, position_embeddings):
+def _fused_layer_forward(self, hidden_states, seq_ctx, position_embeddings, *, recompute=None):
     """Replacement for ``MoEDecoderLayer._forward`` (``moe_decoder_layer.py:392-488``): the attention half is the
-    reference's own modules (``_pre_moe_forward`` lines 634-666), the MoE half one fused autograd node."""
+    reference's own modules (``_pre_moe_forward`` lines 634-666), the MoE half one fused autograd node.  ``recompute`` is
+    bound by :func:`convert_model`."""
     residual = hidden_states
     hidden_states = self.input_layernorm(hidden_states)
     attn_outputs = self.self_attn(hidden_states=hidden_states, position_embeddings=position_embeddings, seq_ctx=seq_ctx)
@@ -123,7 +154,6 @@ def _fused_layer_forward(self, hidden_states, seq_ctx, position_embeddings):
         if seq_ctx.offload_rollout_routed_experts and ids.device != hidden_states.device:
             ids = ids.contiguous().to(hidden_states.device)
         opts["rollout_routed_experts"] = ids
-    recompute = vars(self).get(_SAVED, {}).get("recompute")
     if recompute is not None:
         opts["recompute"] = recompute
     out, rr = _fused.fused_moe_block(
@@ -133,6 +163,12 @@ def _fused_layer_forward(self, hidden_states, seq_ctx, position_embeddings):
         hidden_factor=self.hidden_factor, scoring_func=router.scoring_func, **opts,
     )
     return out, rr["logits"], rr["router_weights"], rr["topk_ids"]
+
+
+def _is_moe_layer(layer: nn.Module) -> bool:
+    # the layer itself, not a wrapper that forwards attribute reads to it (torch's CheckpointWrapper under the
+    # reference's fully_shard does): `dispatcher` is a plain attribute, `gate` / `experts` are sub-modules
+    return "dispatcher" in vars(layer) and "gate" in layer._modules and "experts" in layer._modules
 
 
 def convert_model(model: nn.Module, *, swiglu: bool = True, fused: bool = False, ep: "bool | str" = False,
@@ -150,9 +186,7 @@ def convert_model(model: nn.Module, *, swiglu: bool = True, fused: bool = False,
         raise ValueError(f"convert_model: recompute={recompute!r} applies to the fused nodes: it needs fused=True")
     n = 0
     for layer in model.modules():
-        # the layer itself, not a wrapper that forwards attribute reads to it (torch's CheckpointWrapper under the
-        # reference's fully_shard does): `dispatcher` is a plain attribute, `gate` / `experts` are sub-modules
-        if not ("dispatcher" in vars(layer) and "gate" in layer._modules and "experts" in layer._modules):
+        if not _is_moe_layer(layer):
             continue
         disp = layer.dispatcher
         kind = type(disp).__name__
@@ -162,58 +196,37 @@ def convert_model(model: nn.Module, *, swiglu: bool = True, fused: bool = False,
             # ep > 1 (reference key dispatcher="all2all", module/dispatcher/__init__.py:30-96): same six phases on our ops
             from .ep_dispatcher import All2AllDispatcher, PeerAll2AllDispatcher
 
-            saved: dict[str, Any] = {"dispatcher": disp, "router": layer.gate.router}
-            layer.dispatcher = (PeerAll2AllDispatcher if ep == "peer" else All2AllDispatcher)(
-                n_routed_experts=disp._n_routed_experts, process_group=disp._process_group,
-                training_dtype=disp._training_dtype, generate_dtype=disp._generate_dtype,
-            )
+            dispatcher_cls = PeerAll2AllDispatcher if ep == "peer" else All2AllDispatcher
         elif kind == "NaiveDispatcher":
-            saved = {"dispatcher": disp, "router": layer.gate.router}
-            layer.dispatcher = FusedDispatcher(
-                n_routed_experts=disp._n_routed_experts, process_group=disp._process_group,
-                training_dtype=disp._training_dtype, generate_dtype=disp._generate_dtype,
-            )
+            dispatcher_cls = FusedDispatcher
         else:
             continue  # DeepEP / AGRS / ExpertTP dispatchers are left alone
-        try:
-            layer.gate.router = _convert_router(layer.gate.router)
-        except Exception:
-            layer.dispatcher = disp  # roll the layer back before the error leaves
-            raise
+        # every replacement is built before the first is set: a router that fails to convert leaves the layer whole
+        layer_names = {"dispatcher": dispatcher_cls(
+            n_routed_experts=disp._n_routed_experts, process_group=disp._process_group,
+            training_dtype=disp._training_dtype, generate_dtype=disp._generate_dtype,
+        )}
+        router = _convert_router(layer.gate.router)
+        if fused and kind == "NaiveDispatcher" and _fused_eligible(layer):  # an instance attribute shadows the class method
+            layer_names["_forward"] = types.MethodType(functools.partial(_fused_layer_forward, recompute=recompute), layer)
+        _rebind(layer, **layer_names)
+        _rebind(layer.gate, router=router)
         if swiglu and getattr(layer.experts, "moe_act", None) is not None and getattr(layer.experts.moe_act, "__name__", "") == "native_swiglu":
-            saved["moe_act"] = layer.experts.moe_act
-            layer.experts.moe_act = ops.swiglu
-        if fused and kind == "NaiveDispatcher" and _fused_eligible(layer):
-            saved["fused_forward"] = True
-            saved["recompute"] = recompute
-            layer._forward = types.MethodType(_fused_layer_forward, layer)  # instance attribute shadows the class method
-        setattr(layer, _SAVED, saved)
+            _rebind(layer.experts, moe_act=ops.swiglu)
         n += 1
     if n:
         mgl = importlib.import_module("xtuner.v1.module.grouped_linear.moe_group_linear")
-        if not hasattr(mgl, _SAVED):
-            setattr(mgl, _SAVED, mgl.group_gemm)
-        mgl.group_gemm = _group_gemm_dispatch(getattr(mgl, _SAVED))
+        _rebind(mgl, group_gemm=_group_gemm_dispatch(mgl.group_gemm))
     return n
 
 
 def restore_model(model: nn.Module) -> None:
     for layer in model.modules():
-        saved = vars(layer).get(_SAVED)  # the layer's own attribute, not one a wrapper forwards
-        if not saved:
-            continue
-        layer.dispatcher = saved["dispatcher"]
-        layer.gate.router = saved["router"]
-        if "moe_act" in saved:
-            layer.experts.moe_act = saved["moe_act"]
-        if saved.get("fused_forward"):
-            del layer._forward
-        delattr(layer, _SAVED)
+        if _is_moe_layer(layer):
+            for owner in (layer, layer.gate, layer.experts):
+                _restore(owner)
     try:
-        mgl = importlib.import_module("xtuner.v1.module.grouped_linear.moe_group_linear")
-        if hasattr(mgl, _SAVED):
-            mgl.group_gemm = getattr(mgl, _SAVED)
-            delattr(mgl, _SAVED)
+        _restore(importlib.import_module("xtuner.v1.module.grouped_linear.moe_group_linear"))
     except ImportError:
         pass
 
@@ -247,17 +260,11 @@ def install_ulysses() -> None:
     SP block of ``MultiHeadAttention.forward`` (``mha.py:365-390,421-427``) uses the peer-memory exchange."""
     from .comm import ulysses_all_to_all
 
-    mha = importlib.import_module("xtuner.v1.module.attention.mha")
-    if not hasattr(mha, _SAVED):
-        setattr(mha, _SAVED, mha.ulysses_all_to_all)
-    mha.ulysses_all_to_all = ulysses_all_to_all
+    _rebind(importlib.import_module("xtuner.v1.module.attention.mha"), ulysses_all_to_all=ulysses_all_to_all)
 
 
 def uninstall_ulysses() -> None:
-    mha = importlib.import_module("xtuner.v1.module.attention.mha")
-    if hasattr(mha, _SAVED):
-        mha.ulysses_all_to_all = getattr(mha, _SAVED)
-        delattr(mha, _SAVED)
+    _restore(importlib.import_module("xtuner.v1.module.attention.mha"))
 
 
 # ======================================================================================================
@@ -298,10 +305,7 @@ def install_lm_head_loss() -> None:
 
     Opt-in because it changes one output: like chunk mode, the served calls return ``(loss, (None, {}))``, so in eager
     mode the fp32 logits that the reference returns, and that end up in ``MoEModelOutputs.logits``, are not produced."""
-    ce = importlib.import_module("xtuner.v1.loss.ce_loss")
-    cls = ce.LMHeadLossContext
-    if _SAVED in vars(cls):
-        return
+    cls = importlib.import_module("xtuner.v1.loss.ce_loss").LMHeadLossContext
     orig_eager, orig_chunk = vars(cls)["eager_mode"], vars(cls)["chunk_mode"]
 
     def eager_mode(self, hidden_states, head_weight, head_bias, loss_kwargs):
@@ -317,16 +321,11 @@ def install_lm_head_loss() -> None:
         return orig_chunk(self, hidden_states, head_weight, head_bias, loss_kwargs)
 
     eager_mode.__wrapped__, chunk_mode.__wrapped__ = orig_eager, orig_chunk
-    setattr(cls, _SAVED, (orig_eager, orig_chunk))
-    cls.eager_mode, cls.chunk_mode = eager_mode, chunk_mode
+    _rebind(cls, eager_mode=eager_mode, chunk_mode=chunk_mode)
 
 
 def uninstall_lm_head_loss() -> None:
-    ce = importlib.import_module("xtuner.v1.loss.ce_loss")
-    cls = ce.LMHeadLossContext
-    if _SAVED in vars(cls):
-        cls.eager_mode, cls.chunk_mode = vars(cls)[_SAVED]
-        delattr(cls, _SAVED)
+    _restore(importlib.import_module("xtuner.v1.loss.ce_loss").LMHeadLossContext)
 
 
 # ======================================================================================================
@@ -377,8 +376,6 @@ def install_rl_lm_head() -> None:
     lp_cls = importlib.import_module("xtuner.v1.loss.rl_loss").LogProbContext
     grpo_mod = importlib.import_module("xtuner.v1.rl.loss.grpo_loss")
     grpo_cls = grpo_mod.GRPOLossContext
-    if _SAVED in vars(grpo_cls):
-        return
     lp_loss_fn, lp_chunk_mode = vars(lp_cls)["loss_fn"], vars(lp_cls)["chunk_mode"]
     grpo_loss_fn = vars(grpo_cls)["loss_fn"]
 
@@ -413,21 +410,13 @@ def install_rl_lm_head() -> None:
 
     logprob_loss_fn.__wrapped__, logprob_chunk_mode.__wrapped__, grpo_loss.__wrapped__ = (lp_loss_fn, lp_chunk_mode,
                                                                                           grpo_loss_fn)
-    setattr(lp_cls, _SAVED, (lp_loss_fn, lp_chunk_mode))
-    setattr(grpo_cls, _SAVED, (grpo_loss_fn,))
-    lp_cls.loss_fn, lp_cls.chunk_mode = logprob_loss_fn, logprob_chunk_mode
-    grpo_cls.loss_fn = grpo_loss
+    if _SAVED not in vars(grpo_cls) and _rebind(lp_cls, loss_fn=logprob_loss_fn, chunk_mode=logprob_chunk_mode):
+        _rebind(grpo_cls, loss_fn=grpo_loss)  # both classes or neither
 
 
 def uninstall_rl_lm_head() -> None:
-    lp_cls = importlib.import_module("xtuner.v1.loss.rl_loss").LogProbContext
-    grpo_cls = importlib.import_module("xtuner.v1.rl.loss.grpo_loss").GRPOLossContext
-    if _SAVED in vars(lp_cls):
-        lp_cls.loss_fn, lp_cls.chunk_mode = vars(lp_cls)[_SAVED]
-        delattr(lp_cls, _SAVED)
-    if _SAVED in vars(grpo_cls):
-        (grpo_cls.loss_fn,) = vars(grpo_cls)[_SAVED]
-        delattr(grpo_cls, _SAVED)
+    _restore(importlib.import_module("xtuner.v1.loss.rl_loss").LogProbContext)
+    _restore(importlib.import_module("xtuner.v1.rl.loss.grpo_loss").GRPOLossContext)
 
 
 # ======================================================================================================
@@ -456,8 +445,6 @@ def install_fp8_cast() -> None:
     the reference's functions (``tests/test_plugin_reference_cpu.py``); the two together have not run inside an fp8 training
     step (the reference's fp8 grouped GEMM wheel is absent here)."""
     fu = importlib.import_module("xtuner.v1.float8.fsdp_utils")
-    if hasattr(fu, _SAVED):
-        return
     orig_cast, orig_scales = fu.cast_to_per_block_fp8_with_scales, fu.tensor_to_per_block_fp8_scales
 
     def cast_to_per_block_fp8_with_scales(tensor, scales, block_size=128, float8_dtype=torch.float8_e4m3fn):
@@ -471,23 +458,17 @@ def install_fp8_cast() -> None:
             return ops.fp8_block_scales(local, block_size)
         return orig_scales(tensor, reduce_mesh, float8_dtype, block_size)
 
-    setattr(fu, _SAVED, (orig_cast, orig_scales))
-    fu.cast_to_per_block_fp8_with_scales = cast_to_per_block_fp8_with_scales
-    fu.tensor_to_per_block_fp8_scales = tensor_to_per_block_fp8_scales
+    _rebind(fu, cast_to_per_block_fp8_with_scales=cast_to_per_block_fp8_with_scales,
+            tensor_to_per_block_fp8_scales=tensor_to_per_block_fp8_scales)
 
 
 def uninstall_fp8_cast() -> None:
-    fu = importlib.import_module("xtuner.v1.float8.fsdp_utils")
-    if hasattr(fu, _SAVED):
-        fu.cast_to_per_block_fp8_with_scales, fu.tensor_to_per_block_fp8_scales = getattr(fu, _SAVED)
-        delattr(fu, _SAVED)
+    _restore(importlib.import_module("xtuner.v1.float8.fsdp_utils"))
 
 
 # ======================================================================================================
 # q/k RMSNorm + rotary embedding in front of the attention (SURVEY.md §8f-3)
 # ======================================================================================================
-
-_QK_SAVED = "_xtuner_b200_qk_saved"
 
 
 def _qk_layer_eligible(attn: nn.Module, apply_rotary_pos_emb_cuda) -> bool:
@@ -550,29 +531,23 @@ def install_qk_norm_rope(model: nn.Module) -> int:
     rope = importlib.import_module("xtuner.v1.ops.rotary_emb").apply_rotary_pos_emb_cuda
     n = 0
     for attn in model.modules():
-        if not isinstance(attn, mha.MultiHeadAttention) or _QK_SAVED in vars(attn) or not _qk_layer_eligible(attn, rope):
+        if not isinstance(attn, mha.MultiHeadAttention) or _SAVED in vars(attn) or not _qk_layer_eligible(attn, rope):
             continue
-        orig = attn.apply_rotary_emb
-        norms = None
+        norms = (attn.q_norm.forward, attn.k_norm.forward) if attn.qk_norm else None
+        _rebind(attn, apply_rotary_emb=_qk_rope_closure(attn, attn.apply_rotary_emb, norms))
         if attn.qk_norm:
-            norms = (attn.q_norm.forward, attn.k_norm.forward)
-            attn.q_norm.forward = _identity
-            attn.k_norm.forward = _identity
-        attn.apply_rotary_emb = _qk_rope_closure(attn, orig, norms)
-        setattr(attn, _QK_SAVED, orig)
+            _rebind(attn.q_norm, forward=_identity)
+            _rebind(attn.k_norm, forward=_identity)
         n += 1
     return n
 
 
 def uninstall_qk_norm_rope(model: nn.Module) -> None:
+    mha = importlib.import_module("xtuner.v1.module.attention.mha")
     for attn in model.modules():
-        if _QK_SAVED not in vars(attn):
-            continue
-        attn.apply_rotary_emb = vars(attn)[_QK_SAVED]
-        if attn.qk_norm:
-            del attn.q_norm.forward
-            del attn.k_norm.forward
-        delattr(attn, _QK_SAVED)
+        if isinstance(attn, mha.MultiHeadAttention):
+            for owner in (attn, attn.q_norm, attn.k_norm) if attn.qk_norm else (attn,):
+                _restore(owner)
 
 
 # ======================================================================================================
@@ -607,8 +582,6 @@ def install_moe_aux_loss() -> None:
     aux_mod = importlib.import_module("xtuner.v1.loss.aux_loss")
     moe_loss = importlib.import_module("xtuner.v1.loss.moe_loss")
     cls = aux_mod.AuxLossContext
-    if _SAVED in vars(cls):
-        return
     orig = vars(cls)["accumulate"]
     classes = (cls, moe_loss.BalancingLossContext, moe_loss.ZLossContext)
 
@@ -641,12 +614,8 @@ def install_moe_aux_loss() -> None:
         return hidden_states
 
     accumulate.__wrapped__ = orig
-    setattr(cls, _SAVED, orig)
-    cls.accumulate = accumulate
+    _rebind(cls, accumulate=accumulate)
 
 
 def uninstall_moe_aux_loss() -> None:
-    cls = importlib.import_module("xtuner.v1.loss.aux_loss").AuxLossContext
-    if _SAVED in vars(cls):
-        cls.accumulate = vars(cls)[_SAVED]
-        delattr(cls, _SAVED)
+    _restore(importlib.import_module("xtuner.v1.loss.aux_loss").AuxLossContext)
