@@ -210,9 +210,8 @@ extern "C" int xtb_peer_barrier(void* const* signal_pad_ptrs_dev, int rank, int 
   XTB_CHECK_ARG(world >= 1 && world <= 64 && rank >= 0 && rank < world && channel >= 0, "xtb_peer_barrier: bad rank/world");
   XTB_ENSURE_CTX(signal_pad_ptrs_dev);
   if (world == 1) return XTB_OK;
-  peer_barrier_kernel<<<1, 64, 0, as_stream(stream)>>>(reinterpret_cast<uint32_t* const*>(signal_pad_ptrs_dev), rank,
-                                                      world, channel);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(peer_barrier_kernel, dim3(1), dim3(64), 0, as_stream(stream), false,
+             reinterpret_cast<uint32_t* const*>(signal_pad_ptrs_dev), rank, world, channel);
   return XTB_OK;
 }
 
@@ -236,9 +235,8 @@ extern "C" int xtb_a2a_pull(void* const* peer_in_ptrs_dev, void* out, int rank, 
   const long long total = n_o * n_x * n_m * a.row_vec;
   const int per_src = max(1, min((int)((total + 256 * 8 - 1) / (256 * 8)), max(1, sm_count() * 2 / world)));
   dim3 grid(per_src, world);
-  a2a_pull_kernel<<<grid, 256, 0, as_stream(stream)>>>(reinterpret_cast<const uint4* const*>(peer_in_ptrs_dev),
-                                                      static_cast<uint4*>(out), a);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(a2a_pull_kernel, grid, dim3(256), 0, as_stream(stream), false,
+             reinterpret_cast<const uint4* const*>(peer_in_ptrs_dev), static_cast<uint4*>(out), a);
   return XTB_OK;
 }
 
@@ -251,11 +249,8 @@ extern "C" int xtb_allgather_push(const void* local_in, void* const* peer_out_pt
   if (n_local_elems == 0) return XTB_OK;
   const long long n_vec = n_local_elems / 8;
   const int blocks = comm_blocks(n_vec);
-  if (in_is_f32)
-    allgather_push_kernel<true><<<blocks, 256, 0, as_stream(stream)>>>(local_in, reinterpret_cast<uint4* const*>(peer_out_ptrs_dev), rank, world, n_vec);
-  else
-    allgather_push_kernel<false><<<blocks, 256, 0, as_stream(stream)>>>(local_in, reinterpret_cast<uint4* const*>(peer_out_ptrs_dev), rank, world, n_vec);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(in_is_f32 ? allgather_push_kernel<true> : allgather_push_kernel<false>, dim3(blocks), dim3(256), 0,
+             as_stream(stream), false, local_in, reinterpret_cast<uint4* const*>(peer_out_ptrs_dev), rank, world, n_vec);
   return XTB_OK;
 }
 
@@ -268,11 +263,9 @@ extern "C" int xtb_reduce_scatter_pull(void* const* peer_in_ptrs_dev, void* out,
   if (n_local_elems == 0) return XTB_OK;
   const long long n_vec = n_local_elems / 8;
   const int blocks = comm_blocks(n_vec);
-  if (out_is_f32)
-    reduce_scatter_pull_kernel<true><<<blocks, 256, 0, as_stream(stream)>>>(reinterpret_cast<const uint4* const*>(peer_in_ptrs_dev), out, rank, world, n_vec, scale);
-  else
-    reduce_scatter_pull_kernel<false><<<blocks, 256, 0, as_stream(stream)>>>(reinterpret_cast<const uint4* const*>(peer_in_ptrs_dev), out, rank, world, n_vec, scale);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(out_is_f32 ? reduce_scatter_pull_kernel<true> : reduce_scatter_pull_kernel<false>, dim3(blocks), dim3(256),
+             0, as_stream(stream), false, reinterpret_cast<const uint4* const*>(peer_in_ptrs_dev), out, rank, world, n_vec,
+             scale);
   return XTB_OK;
 }
 
@@ -284,9 +277,8 @@ extern "C" int xtb_allreduce_pull_f32(void* const* peer_in_ptrs_dev, void* out, 
   XTB_ENSURE_CTX(out);
   if (n_elems == 0) return XTB_OK;
   const long long n_vec = n_elems / 4;
-  allreduce_pull_f32_kernel<<<comm_blocks(n_vec), 256, 0, as_stream(stream)>>>(
-      reinterpret_cast<const float4* const*>(peer_in_ptrs_dev), static_cast<float4*>(out), world, n_vec, scale);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(allreduce_pull_f32_kernel, dim3(comm_blocks(n_vec)), dim3(256), 0, as_stream(stream), false,
+             reinterpret_cast<const float4* const*>(peer_in_ptrs_dev), static_cast<float4*>(out), world, n_vec, scale);
   return XTB_OK;
 }
 

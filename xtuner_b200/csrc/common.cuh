@@ -30,14 +30,14 @@ extern std::atomic<int64_t> g_launch_count;
                          __LINE__);                                                                  \
   } while (0)
 
-// call right after a <<<>>> launch
-#define XTB_LAUNCH_OK()                        \
-  do {                                         \
-    ::xtb::g_launch_count.fetch_add(1);        \
-    XTB_CUDA(cudaGetLastError());              \
-  } while (0)
-
 inline cudaStream_t as_stream(xtb_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
+
+// Raises `kernel`'s dynamic shared-memory limit on the current device to at least `bytes`.  The default limit is 48 KB
+// less the kernel's static shared memory, so a kernel with static shared memory can need this below 48 KB of dynamic
+// memory.  CUDA keeps the limit per device: the limit is recorded per (kernel, device), read from the kernel on the
+// first call and raised only when a launch needs more; after the first call for a pair only a lookup remains.
+// Thread-safe (autograd runs the backward on its own thread).  Returns XTB_OK or an error status.
+int smem_opt_in(const void* kernel, size_t bytes);
 
 int sm_count();  // cached multiProcessorCount of the current device
 
@@ -60,7 +60,7 @@ int lm_head_logits_ce(const void* h, const void* w, const int64_t* tokens_per_ex
 // ---- device helpers ------------------------------------------------------------------------------
 #ifdef __CUDACC__
 
-// Programmatic dependent launch.  A kernel launched through launch_pdl() may become resident while
+// Programmatic dependent launch.  A kernel launched with XTB_LAUNCH(..., pdl = true, ...) may become resident while
 // its predecessor in the stream is still draining (its CTAs take over SMs as the predecessor's CTAs retire, hiding launch
 // latency and set-up); it must not touch global memory before pdl_sync().  Launched without the attribute, both
 // instructions are no-ops.
@@ -75,8 +75,17 @@ __device__ __forceinline__ void pdl_sync() {
   pdl_wait();
 }
 
+// Every kernel of the library is launched here: raises the kernel's dynamic shared-memory limit when `smem` is above
+// it (smem_opt_in), launches it (programmatic dependent launch exactly when `pdl` is set: only kernels that wait with
+// pdl_sync() / pdl_wait() may take it), counts the launch and checks for a launch error.  Use XTB_LAUNCH, which
+// supplies the call site and returns from the caller on error.
 template <typename... P, typename... A>
-inline cudaError_t launch_pdl(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+inline int launch(const char* file, int line, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem,
+                  cudaStream_t st, bool pdl, A&&... args) {
+  if (smem > 0) {
+    const int rc = smem_opt_in(reinterpret_cast<const void*>(kernel), smem);
+    if (rc != XTB_OK) return rc;
+  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -86,9 +95,23 @@ inline cudaError_t launch_pdl(void (*kernel)(P...), dim3 grid, dim3 block, size_
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, P(args)...);
+  cfg.numAttrs = pdl ? 1 : 0;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, P(args)...);
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // the refusal is not sticky: clear it, or the next launch's check would report it again
+    return fail(XTB_ERR_CUDA, "kernel launch refused: %s (%s:%d)", cudaGetErrorString(e), file, line);
+  }
+  g_launch_count.fetch_add(1);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(XTB_ERR_CUDA, "kernel launch: %s (%s:%d)", cudaGetErrorString(e), file, line);
+  return XTB_OK;
 }
+
+#define XTB_LAUNCH(...)                                                  \
+  do {                                                                   \
+    const int _rc = ::xtb::launch(__FILE__, __LINE__, __VA_ARGS__);      \
+    if (_rc != XTB_OK) return _rc;                                       \
+  } while (0)
 
 constexpr int kWarp = 32;
 

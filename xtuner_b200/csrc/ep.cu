@@ -250,8 +250,8 @@ extern "C" int xtb_ep_write_header(const int64_t* tokens_per_expert, void* heade
   XTB_CHECK_ARG(tokens_per_expert && header, "xtb_ep_write_header: null pointer");
   XTB_CHECK_ARG(E > 0, "xtb_ep_write_header: bad E=%d", E);
   XTB_ENSURE_CTX(header);
-  ep_write_header_kernel<<<1, 256, 0, as_stream(stream)>>>(tokens_per_expert, static_cast<int32_t*>(header), E);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(ep_write_header_kernel, dim3(1), dim3(256), 0, as_stream(stream), false, tokens_per_expert,
+             static_cast<int32_t*>(header), E);
   return XTB_OK;
 }
 
@@ -268,17 +268,10 @@ extern "C" int xtb_ep_pull_to_experts(void* const* peer_ptrs_dev, const int32_t*
   a.me = rank; a.world = world; a.E = E; a.E_loc = E / world;
   a.row_vec = (int)(row_bytes / 16); a.hdr_vec = hdr_bytes / 16; a.cap_rows = (int)cap_rows; a.m_rows = 0;
   const size_t smem = ep_smem_bytes(world, E, a.E_loc);
-  static bool attr = false;
-  if (!attr) {
-    XTB_CUDA(cudaFuncSetAttribute(ep_pull_to_experts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    XTB_CUDA(cudaFuncSetAttribute(ep_pull_to_sources_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    attr = true;
-  }
   XTB_CHECK_ARG(smem <= 96 * 1024, "xtb_ep_pull_to_experts: count tables need %zu bytes of shared memory", smem);
-  ep_pull_to_experts_kernel<<<sm_count() * 2, 256, smem, as_stream(stream)>>>(
-      reinterpret_cast<const uint4* const*>(peer_ptrs_dev), cnt_all_in, cnt_all_out, static_cast<uint4*>(out),
-      tokens_per_expert_local, status, a);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(ep_pull_to_experts_kernel, dim3(sm_count() * 2), dim3(256), smem, as_stream(stream), false,
+             reinterpret_cast<const uint4* const*>(peer_ptrs_dev), cnt_all_in, cnt_all_out, static_cast<uint4*>(out),
+             tokens_per_expert_local, status, a);
   return XTB_OK;
 }
 
@@ -296,15 +289,8 @@ extern "C" int xtb_ep_pull_to_sources(void* const* peer_ptrs_dev, const int32_t*
   a.me = rank; a.world = world; a.E = E; a.E_loc = E / world;
   a.row_vec = (int)(row_bytes / 16); a.hdr_vec = hdr_bytes / 16; a.cap_rows = (int)cap_rows; a.m_rows = (int)m_rows;
   const size_t smem = ep_smem_bytes(world, E, a.E_loc);
-  static bool attr = false;
-  if (!attr) {
-    XTB_CUDA(cudaFuncSetAttribute(ep_pull_to_experts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    XTB_CUDA(cudaFuncSetAttribute(ep_pull_to_sources_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    attr = true;
-  }
   XTB_CHECK_ARG(smem <= 96 * 1024, "xtb_ep_pull_to_sources: count tables need %zu bytes of shared memory", smem);
-  ep_pull_to_sources_kernel<<<sm_count() * 2, 256, smem, as_stream(stream)>>>(
-      reinterpret_cast<const uint4* const*>(peer_ptrs_dev), cnt_all, static_cast<uint4*>(out), a);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(ep_pull_to_sources_kernel, dim3(sm_count() * 2), dim3(256), smem, as_stream(stream), false,
+             reinterpret_cast<const uint4* const*>(peer_ptrs_dev), cnt_all, static_cast<uint4*>(out), a);
   return XTB_OK;
 }

@@ -116,9 +116,8 @@ extern "C" int xtb_fp8_per_tile_quant(const void* x_bf16, void* q_e4m3, float* s
   XTB_ENSURE_CTX(x_bf16);
   const long long n_tiles = M * (K / 128);
   if (n_tiles == 0) return XTB_OK;
-  fp8_per_tile_quant_kernel<<<(unsigned)((n_tiles + 7) / 8), 256, 0, as_stream(stream)>>>(
-      static_cast<const __nv_bfloat16*>(x_bf16), static_cast<uint8_t*>(q_e4m3), scales, n_tiles);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(fp8_per_tile_quant_kernel, dim3((unsigned)((n_tiles + 7) / 8)), dim3(256), 0, as_stream(stream), false,
+             static_cast<const __nv_bfloat16*>(x_bf16), static_cast<uint8_t*>(q_e4m3), scales, n_tiles);
   return XTB_OK;
 }
 
@@ -131,9 +130,12 @@ extern "C" int xtb_fp8_block_scales(const void* w, int w_is_f32, int64_t nw, int
   XTB_ENSURE_CTX(w);
   if (nw == 0) return XTB_OK;
   dim3 grid(din / 128, dout / 128, (unsigned)nw);
-  if (w_is_f32) fp8_block_kernel<float, false><<<grid, 256, 0, as_stream(stream)>>>(static_cast<const float*>(w), dout, din, scales, nullptr, nullptr);
-  else fp8_block_kernel<__nv_bfloat16, false><<<grid, 256, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(w), dout, din, scales, nullptr, nullptr);
-  XTB_LAUNCH_OK();
+  if (w_is_f32)
+    XTB_LAUNCH(fp8_block_kernel<float, false>, grid, dim3(256), 0, as_stream(stream), false, static_cast<const float*>(w),
+               dout, din, scales, nullptr, nullptr);
+  else
+    XTB_LAUNCH(fp8_block_kernel<__nv_bfloat16, false>, grid, dim3(256), 0, as_stream(stream), false,
+               static_cast<const __nv_bfloat16*>(w), dout, din, scales, nullptr, nullptr);
   return XTB_OK;
 }
 
@@ -146,8 +148,11 @@ extern "C" int xtb_fp8_block_cast(const void* w, int w_is_f32, int64_t nw, int d
   XTB_ENSURE_CTX(w);
   if (nw == 0) return XTB_OK;
   dim3 grid(din / 128, dout / 128, (unsigned)nw);
-  if (w_is_f32) fp8_block_kernel<float, true><<<grid, 256, 0, as_stream(stream)>>>(static_cast<const float*>(w), dout, din, nullptr, scales, static_cast<uint8_t*>(q_e4m3));
-  else fp8_block_kernel<__nv_bfloat16, true><<<grid, 256, 0, as_stream(stream)>>>(static_cast<const __nv_bfloat16*>(w), dout, din, nullptr, scales, static_cast<uint8_t*>(q_e4m3));
-  XTB_LAUNCH_OK();
+  if (w_is_f32)
+    XTB_LAUNCH(fp8_block_kernel<float, true>, grid, dim3(256), 0, as_stream(stream), false, static_cast<const float*>(w),
+               dout, din, nullptr, scales, static_cast<uint8_t*>(q_e4m3));
+  else
+    XTB_LAUNCH(fp8_block_kernel<__nv_bfloat16, true>, grid, dim3(256), 0, as_stream(stream), false,
+               static_cast<const __nv_bfloat16*>(w), dout, din, nullptr, scales, static_cast<uint8_t*>(q_e4m3));
   return XTB_OK;
 }

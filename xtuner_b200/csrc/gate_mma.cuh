@@ -222,18 +222,12 @@ int launch_gate_route_mma(const __nv_bfloat16* x, const float* w, float* logits,
                           void* dispatch_ws, cudaStream_t st, const int64_t* replay_ids, int64_t replay_stride) {
   const size_t smem = (size_t)3 * (H / 32) * 32 * sizeof(uint4);
   if (E > 8 || K > 8 || H % 128 != 0 || smem > 200 * 1024) return -1;
-  static bool attr = false;
-  if (!attr) {
-    XTB_CUDA(cudaFuncSetAttribute(gate_route_mma_kernel<REPLAY>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr = true;
-  }
   PermuteWorkspace pw = carve_permute_workspace(dispatch_ws, E);
   const int n_chunks = n_chunks_of(T);
   const int blocks = max(1, min(2 * sm_count(), n_chunks));
-  XTB_CUDA(launch_pdl(gate_route_mma_kernel<REPLAY>, dim3(blocks), dim3(256), smem, st, x, w, logits, T, H, E, K, scoring,
-                      norm, scaling, rw, tw, ids, ids32, reinterpret_cast<unsigned long long*>(tpe), pw.counts,
-                      pw.expert_start, pw.ticket, n_chunks, replay_ids, replay_stride));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(gate_route_mma_kernel<REPLAY>, dim3(blocks), dim3(256), smem, st, true, x, w, logits, T, H, E, K, scoring,
+             norm, scaling, rw, tw, ids, ids32, reinterpret_cast<unsigned long long*>(tpe), pw.counts, pw.expert_start,
+             pw.ticket, n_chunks, replay_ids, replay_stride);
   return XTB_OK;
 }
 

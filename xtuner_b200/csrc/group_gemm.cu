@@ -486,14 +486,8 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmA
   }
   const CUtensorMap& a2 = ta2 ? *ta2 : ta;
   const CUtensorMap& b2 = tb2 ? *tb2 : tb;
-  static bool attr_set = false;
-  auto kfn = group_gemm_kernel<MODE, BLOCK_N, EPI>;
-  if (!attr_set) {
-    XTB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  XTB_CUDA(launch_pdl(kfn, dim3(sm_count()), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, st, ta, tb, to, to2, a2, b2, args));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(group_gemm_kernel<MODE, BLOCK_N, EPI>, dim3(sm_count()), dim3(kGemmThreads), (size_t)Cfg::kSmemBytes, st,
+             true, ta, tb, to, to2, a2, b2, args);
   return XTB_OK;
 }
 

@@ -2,6 +2,9 @@
 #include <cuda.h>
 
 #include <cstring>
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "common.cuh"
 
@@ -34,6 +37,23 @@ int sm_count() {
   return cached[dev];
 }
 
+int smem_opt_in(const void* kernel, size_t bytes) {
+  int dev = 0;
+  XTB_CUDA(cudaGetDevice(&dev));
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> limits;  // (kernel, device) -> its dynamic shared-memory limit
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = limits.find({kernel, dev});
+  if (it == limits.end()) {
+    cudaFuncAttributes fa;
+    XTB_CUDA(cudaFuncGetAttributes(&fa, kernel));
+    it = limits.emplace(std::make_pair(kernel, dev), (size_t)fa.maxDynamicSharedSizeBytes).first;
+  }
+  if (bytes <= it->second) return XTB_OK;
+  XTB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  it->second = bytes;
+  return XTB_OK;
+}
 
 typedef CUresult (*PFN_ctxGetCurrent)(CUcontext*);
 typedef CUresult (*PFN_ctxSetCurrent)(CUcontext);

@@ -199,17 +199,14 @@ extern "C" int xtb_lm_head_ce(const void* h, const void* w, const int64_t* label
   }
   int64_t* tpe = static_cast<int64_t*>(workspace);
   float2* part = reinterpret_cast<float2*>(static_cast<uint8_t*>(workspace) + kWsHeader);
-  XTB_CUDA(launch_pdl(ce_set_rows_kernel, dim3(1), dim3(32), 0, st, tpe, T));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(ce_set_rows_kernel, dim3(1), dim3(32), 0, st, true, tpe, T);
   int rc = lm_head_logits_ce(h, w, tpe, T, H, V, z_or_G, part, st);
   if (rc) return rc;
-  XTB_CUDA(launch_pdl(ce_row_kernel, dim3((unsigned)T), dim3(kRowThreads), 0, st, static_cast<__nv_bfloat16*>(z_or_G),
-                      static_cast<const float2*>(part), lm_head_ce_vocab_tiles(V), labels, ignore_index, loss_weight, V,
-                      need_grad, row_ce));
-  XTB_LAUNCH_OK();
-  XTB_CUDA(launch_pdl(ce_loss_kernel, dim3(1), dim3(kLossThreads), 0, st, static_cast<const float*>(row_ce), loss_weight,
-                      T, loss));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(ce_row_kernel, dim3((unsigned)T), dim3(kRowThreads), 0, st, true, static_cast<__nv_bfloat16*>(z_or_G),
+             static_cast<const float2*>(part), lm_head_ce_vocab_tiles(V), labels, ignore_index, loss_weight, V,
+             need_grad, row_ce);
+  XTB_LAUNCH(ce_loss_kernel, dim3(1), dim3(kLossThreads), 0, st, true, static_cast<const float*>(row_ce), loss_weight,
+             T, loss);
   if (!need_grad) return XTB_OK;
   if ((rc = xtb_group_gemm_nn(z_or_G, w, tpe, T, V, H, 1, dh, stream))) return rc;
   return xtb_group_gemm_tn(z_or_G, h, tpe, T, V, H, 1, dW, stream);
@@ -234,14 +231,12 @@ extern "C" int xtb_lm_head_logprob(const void* h, const void* w, const int64_t* 
   cudaStream_t st = as_stream(stream);
   int64_t* tpe = static_cast<int64_t*>(workspace);
   float2* part = reinterpret_cast<float2*>(static_cast<uint8_t*>(workspace) + kWsHeader);
-  XTB_CUDA(launch_pdl(ce_set_rows_kernel, dim3(1), dim3(32), 0, st, tpe, T));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(ce_set_rows_kernel, dim3(1), dim3(32), 0, st, true, tpe, T);
   const int rc = lm_head_logits_ce(h, w, tpe, T, H, V, z, part, st);
   if (rc) return rc;
-  XTB_CUDA(launch_pdl(logprob_row_kernel, dim3((unsigned)T), dim3(kRowThreads), 0, st,
-                      static_cast<const __nv_bfloat16*>(z), static_cast<const float2*>(part), lm_head_ce_vocab_tiles(V),
-                      labels, V, logp, reinterpret_cast<float2*>(row_stats)));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(logprob_row_kernel, dim3((unsigned)T), dim3(kRowThreads), 0, st, true,
+             static_cast<const __nv_bfloat16*>(z), static_cast<const float2*>(part), lm_head_ce_vocab_tiles(V),
+             labels, V, logp, reinterpret_cast<float2*>(row_stats));
   return XTB_OK;
 }
 
@@ -267,12 +262,10 @@ extern "C" int xtb_lm_head_logprob_bwd(void* z_or_G, const float* row_stats, con
     return XTB_OK;
   }
   int64_t* tpe = static_cast<int64_t*>(workspace);
-  XTB_CUDA(launch_pdl(ce_set_rows_kernel, dim3(1), dim3(32), 0, st, tpe, T));
-  XTB_LAUNCH_OK();
-  XTB_CUDA(launch_pdl(logprob_grad_row_kernel, dim3((unsigned)T), dim3(kRowThreads), 0, st,
-                      static_cast<__nv_bfloat16*>(z_or_G), reinterpret_cast<const float2*>(row_stats), labels, grad_logp,
-                      V));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(ce_set_rows_kernel, dim3(1), dim3(32), 0, st, true, tpe, T);
+  XTB_LAUNCH(logprob_grad_row_kernel, dim3((unsigned)T), dim3(kRowThreads), 0, st, true,
+             static_cast<__nv_bfloat16*>(z_or_G), reinterpret_cast<const float2*>(row_stats), labels, grad_logp,
+             V);
   int rc;
   if ((rc = xtb_group_gemm_nn(z_or_G, w, tpe, T, V, H, 1, dh, stream))) return rc;
   return xtb_group_gemm_tn(z_or_G, h, tpe, T, V, H, 1, dW, stream);

@@ -233,21 +233,18 @@ extern "C" int xtb_moe_aux_stats(const float* rw, const float* logits, const int
   const int64_t rows = N ? (N + G - 1) / G : 1;
   const int grid = N ? (int)((N + rows - 1) / rows) : 1;
   const AuxWorkspace ws = carve_aux_workspace(workspace, G, E);
-#define XTB_AUXF(LL, JJ)                                                                                               \
-  XTB_CUDA(launch_pdl(moe_aux_stats_kernel<LL, JJ>, dim3(grid), dim3(kAuxThreads), 0, st, rw, logits, ids, N, E, K,    \
-                      rows, ws, tokens_per_expert, rw_sum, z_sum, lse))
-  if (E <= 1) XTB_AUXF(1, 1);
-  else if (E <= 2) XTB_AUXF(2, 1);
-  else if (E <= 4) XTB_AUXF(4, 1);
-  else if (E <= 8) XTB_AUXF(8, 1);
-  else if (E <= 16) XTB_AUXF(16, 1);
-  else if (E <= 32) XTB_AUXF(32, 1);
-  else if (E <= 64) XTB_AUXF(32, 2);
-  else if (E <= 128) XTB_AUXF(32, 4);
-  else if (E <= 256) XTB_AUXF(32, 8);
-  else XTB_AUXF(32, 16);
-#undef XTB_AUXF
-  XTB_LAUNCH_OK();
+  auto* kernel = E <= 1     ? moe_aux_stats_kernel<1, 1>
+                 : E <= 2   ? moe_aux_stats_kernel<2, 1>
+                 : E <= 4   ? moe_aux_stats_kernel<4, 1>
+                 : E <= 8   ? moe_aux_stats_kernel<8, 1>
+                 : E <= 16  ? moe_aux_stats_kernel<16, 1>
+                 : E <= 32  ? moe_aux_stats_kernel<32, 1>
+                 : E <= 64  ? moe_aux_stats_kernel<32, 2>
+                 : E <= 128 ? moe_aux_stats_kernel<32, 4>
+                 : E <= 256 ? moe_aux_stats_kernel<32, 8>
+                            : moe_aux_stats_kernel<32, 16>;
+  XTB_LAUNCH(kernel, dim3(grid), dim3(kAuxThreads), 0, st, true, rw, logits, ids, N, E, K, rows, ws, tokens_per_expert,
+             rw_sum, z_sum, lse);
   return XTB_OK;
 }
 
@@ -262,8 +259,7 @@ extern "C" int xtb_moe_aux_stats_bwd(const float* g_rw_sum, const float* g_z, co
   XTB_ENSURE_CTX(g_rw ? (const void*)g_rw : (const void*)g_logits);
   const int64_t total = N * E;
   const int blocks = (int)min((int64_t)sm_count() * 8, (total + 255) / 256);
-  XTB_CUDA(launch_pdl(moe_aux_stats_bwd_kernel, dim3(blocks), dim3(256), 0, as_stream(stream), g_rw_sum, g_z, logits,
-                      lse, N, E, g_rw, g_logits));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(moe_aux_stats_bwd_kernel, dim3(blocks), dim3(256), 0, as_stream(stream), true, g_rw_sum, g_z, logits,
+             lse, N, E, g_rw, g_logits);
   return XTB_OK;
 }

@@ -448,32 +448,18 @@ extern "C" int xtb_rmsnorm_gate(const void* h_bf16, const float* norm_w_f32, con
                 "xtb_rmsnorm_gate: unsupported H=%d (256, 512, 1024, 2048: the row lives in registers)", H);
   if (!gate_w_f32) {
     // norm only: column-owned streaming kernel, 4 tokens per 256-thread block (one 8-column vector per thread)
-    XTB_CUDA(launch_pdl(rmsnorm_cols_kernel<4>, dim3((T + 3) / 4), dim3(256), 0, st, hp, norm_w_f32, xp, rstd_out, T, H, eps));
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(rmsnorm_cols_kernel<4>, dim3((T + 3) / 4), dim3(256), 0, st, true, hp, norm_w_f32, xp, rstd_out, T, H, eps);
     return XTB_OK;
   }
   const int blocks = min(sm_count(), (T + 15) / 16);
   const size_t smem = ((size_t)E * H + H) * sizeof(float);
   XTB_CHECK_ARG(smem <= 200 * 1024, "xtb_rmsnorm_gate: E*H too large for the fused gate (%zu bytes of smem)", smem);
-#define XTB_RG(R8)                                                                                                   \
-  do {                                                                                                               \
-    static bool attr = false;                                                                                        \
-    if (!attr) {                                                                                                     \
-      XTB_CUDA(cudaFuncSetAttribute(rmsnorm_gate_kernel<8, 2, R8>, cudaFuncAttributeMaxDynamicSharedMemorySize,      \
-                                    200 * 1024));                                                                    \
-      attr = true;                                                                                                   \
-    }                                                                                                                \
-    rmsnorm_gate_kernel<8, 2, R8><<<blocks, 256, smem, st>>>(hp, norm_w_f32, gate_w_f32, xp, rstd_out, logits, T, H, E, \
-                                                             eps);                                                   \
-  } while (0)
-  switch (H / 256) {
-    case 1: XTB_RG(1); break;
-    case 2: XTB_RG(2); break;
-    case 4: XTB_RG(4); break;
-    default: XTB_RG(8); break;
-  }
-#undef XTB_RG
-  XTB_LAUNCH_OK();
+  auto* kernel = H == 256 ? rmsnorm_gate_kernel<8, 2, 1>
+               : H == 512 ? rmsnorm_gate_kernel<8, 2, 2>
+               : H == 1024 ? rmsnorm_gate_kernel<8, 2, 4>
+                           : rmsnorm_gate_kernel<8, 2, 8>;
+  XTB_LAUNCH(kernel, dim3(blocks), dim3(256), smem, st, false, hp, norm_w_f32, gate_w_f32, xp, rstd_out, logits, T, H, E,
+             eps);
   return XTB_OK;
 }
 
@@ -495,33 +481,26 @@ extern "C" int xtb_moe_dispatch_bwd_rmsnorm(const void* g_xperm_bf16, const int3
   cudaStream_t st = as_stream(stream);
   const int blocks = norm_bwd_blocks(T);
   float* partial = g_norm_w ? static_cast<float*>(workspace) : nullptr;
-#define XTB_NBP(KT, TB)                                                                                             \
-  do {                                                                                                               \
-    constexpr size_t smem = (size_t)2 * TB * (KT + 3) * 256 * sizeof(uint4);                                         \
-    static bool attr = false;                                                                                        \
-    if (!attr) {                                                                                                     \
-      XTB_CUDA(cudaFuncSetAttribute(dispatch_bwd_rmsnorm_pipe_kernel<KT, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-      attr = true;                                                                                                   \
-    }                                                                                                                \
-    XTB_CUDA(launch_pdl(dispatch_bwd_rmsnorm_pipe_kernel<KT, TB>, dim3(blocks), dim3(256), smem, st,                 \
-        static_cast<const uint4*>(g_xperm_bf16), row_id_map, static_cast<const uint4*>(g_x_gate_bf16),               \
-        static_cast<const uint4*>(h_bf16), rstd, norm_w_f32, static_cast<const uint4*>(g_res_bf16),                  \
-        static_cast<uint4*>(g_h_bf16), partial, T, H));                                                              \
-  } while (0)
-  if (K == 2) XTB_NBP(2, 2);
-  else if (K == 8) XTB_NBP(8, 1);
-  else
-    XTB_CUDA(launch_pdl(dispatch_bwd_rmsnorm_kernel<4>, dim3(blocks), dim3(256), 0, st,
-                        static_cast<const uint4*>(g_xperm_bf16), row_id_map, static_cast<const uint4*>(g_x_gate_bf16),
-                        static_cast<const uint4*>(h_bf16), rstd, norm_w_f32, static_cast<const uint4*>(g_res_bf16),
-                        static_cast<uint4*>(g_h_bf16), partial, T, K, H));
-#undef XTB_NBP
-  XTB_LAUNCH_OK();
+  const auto* gx = static_cast<const uint4*>(g_xperm_bf16);
+  const auto* gxg = static_cast<const uint4*>(g_x_gate_bf16);
+  const auto* hv = static_cast<const uint4*>(h_bf16);
+  const auto* gres = static_cast<const uint4*>(g_res_bf16);
+  auto* gh = static_cast<uint4*>(g_h_bf16);
+  if (K == 2 || K == 8) {
+    // <KT, TB>: two stages of TB token groups, (KT + 3) 16-byte vectors per thread each
+    auto* kernel = K == 2 ? dispatch_bwd_rmsnorm_pipe_kernel<2, 2> : dispatch_bwd_rmsnorm_pipe_kernel<8, 1>;
+    const int TB = K == 2 ? 2 : 1;
+    const size_t smem = (size_t)2 * TB * (K + 3) * 256 * sizeof(uint4);
+    XTB_LAUNCH(kernel, dim3(blocks), dim3(256), smem, st, true, gx, row_id_map, gxg, hv, rstd, norm_w_f32, gres, gh,
+               partial, T, H);
+  } else {
+    XTB_LAUNCH(dispatch_bwd_rmsnorm_kernel<4>, dim3(blocks), dim3(256), 0, st, true, gx, row_id_map, gxg, hv, rstd,
+               norm_w_f32, gres, gh, partial, T, K, H);
+  }
   if (g_norm_w) {
     // H outputs, up to 2 partial rows per SM: 32 warps per block put all of a lane's ~9 loads in flight at once
-    XTB_CUDA(launch_pdl(reduce_partial_rows_kernel<32>, dim3((H + 31) / 32), dim3(1024), 0, st, (const float*)partial, g_norm_w,
-                        blocks, (int64_t)H));
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(reduce_partial_rows_kernel<32>, dim3((H + 31) / 32), dim3(1024), 0, st, true, (const float*)partial,
+               g_norm_w, blocks, (int64_t)H);
   }
   return XTB_OK;
 }

@@ -458,10 +458,8 @@ static int permute_impl(const void* x, const int32_t* ids, int T, int K, int E, 
     const int wpb = 8;
     const int blocks = max(1, min((n_chunks + wpb - 1) / wpb, sm_count() * 4));
     const size_t smem = (size_t)wpb * E * sizeof(int);
-    permute_count_scan_kernel<<<blocks, wpb * 32, smem, st>>>(
-        ids, T, K, E, n_chunks, w.counts, w.expert_start,
-        reinterpret_cast<unsigned long long*>(tokens_per_expert), w.ticket);
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(permute_count_scan_kernel, dim3(blocks), dim3(wpb * 32), smem, st, false, ids, T, K, E, n_chunks, w.counts,
+               w.expert_start, reinterpret_cast<unsigned long long*>(tokens_per_expert), w.ticket);
   }
   {
     const size_t smem = (size_t)(kChunkTokens + kSubTokens) * K * sizeof(int);
@@ -471,21 +469,13 @@ static int permute_impl(const void* x, const int32_t* ids, int T, int K, int E, 
     // H >= 12784) through registers
     const size_t smem_bulk = (size_t)kSubTokens * row_bytes + kSubTokens * sizeof(uint64_t) + smem;
     if (smem_bulk <= 200 * 1024) {
-      static bool attr = false;
-      if (!attr) {
-        XTB_CUDA(cudaFuncSetAttribute(permute_scatter_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        attr = true;
-      }
-      XTB_CUDA(launch_pdl(permute_scatter_bulk_kernel, dim3(n_sub), dim3(128), smem_bulk, st, static_cast<const uint8_t*>(x), ids, T, K, E, (uint32_t)row_bytes,
-                                                                  w.counts, w.expert_start, static_cast<uint8_t*>(permuted),
-                                                                  row_id_map, sorted_indices));
+      XTB_LAUNCH(permute_scatter_bulk_kernel, dim3(n_sub), dim3(128), smem_bulk, st, true, static_cast<const uint8_t*>(x),
+                 ids, T, K, E, (uint32_t)row_bytes, w.counts, w.expert_start, static_cast<uint8_t*>(permuted), row_id_map,
+                 sorted_indices);
     } else {
-      XTB_CUDA(launch_pdl(permute_scatter_kernel, dim3(n_sub), dim3(128), smem, st, static_cast<const uint4*>(x), ids, T, K, E, row_vec,
-                                                                w.counts, w.expert_start,
-                                                                static_cast<uint4*>(permuted), row_id_map,
-                                                                sorted_indices));
+      XTB_LAUNCH(permute_scatter_kernel, dim3(n_sub), dim3(128), smem, st, true, static_cast<const uint4*>(x), ids, T, K,
+                 E, row_vec, w.counts, w.expert_start, static_cast<uint4*>(permuted), row_id_map, sorted_indices);
     }
-    XTB_LAUNCH_OK();
   }
   return XTB_OK;
 }
@@ -518,17 +508,13 @@ static int combine_impl(const char* entry, const void* y_bf16, const int32_t* ro
   const auto* y = static_cast<const uint4*>(y_bf16);
   const auto* res = static_cast<const uint4*>(residual_bf16);
   auto* out = static_cast<uint4*>(out_bf16);
-#define XTB_UNPERMUTE(KT) XTB_CUDA(launch_pdl(unpermute_kernel<KT>, dim3(blocks), dim3(256), 0, st, y, row_id_map, probs, T, K, row_vec, out, res, hidden_factor))
-  switch (K) {
-    case 1: XTB_UNPERMUTE(1); break;
-    case 2: XTB_UNPERMUTE(2); break;
-    case 4: XTB_UNPERMUTE(4); break;
-    case 6: XTB_UNPERMUTE(6); break;
-    case 8: XTB_UNPERMUTE(8); break;
-    default: XTB_UNPERMUTE(0); break;
-  }
-#undef XTB_UNPERMUTE
-  XTB_LAUNCH_OK();
+  auto* kernel = K == 1 ? unpermute_kernel<1>
+               : K == 2 ? unpermute_kernel<2>
+               : K == 4 ? unpermute_kernel<4>
+               : K == 6 ? unpermute_kernel<6>
+               : K == 8 ? unpermute_kernel<8>
+                        : unpermute_kernel<0>;
+  XTB_LAUNCH(kernel, dim3(blocks), dim3(256), 0, st, true, y, row_id_map, probs, T, K, row_vec, out, res, hidden_factor);
   return XTB_OK;
 }
 
@@ -553,10 +539,9 @@ extern "C" int xtb_moe_unpermute_bwd(const void* grad_out_bf16, const void* y_fw
   XTB_ENSURE_CTX(grad_out_bf16);
   if (T == 0) return XTB_OK;
   cudaStream_t st = as_stream(stream);
-  XTB_CUDA(launch_pdl(unpermute_bwd_kernel, dim3((T + 7) / 8), dim3(256), 0, st, static_cast<const uint4*>(grad_out_bf16),
-                                                    static_cast<const uint4*>(y_fwd_bf16), row_id_map, probs, T, K,
-                                                    H / 8, static_cast<uint4*>(act_grad_bf16), prob_grad));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(unpermute_bwd_kernel, dim3((T + 7) / 8), dim3(256), 0, st, true, static_cast<const uint4*>(grad_out_bf16),
+             static_cast<const uint4*>(y_fwd_bf16), row_id_map, probs, T, K, H / 8, static_cast<uint4*>(act_grad_bf16),
+             prob_grad);
   return XTB_OK;
 }
 
@@ -568,9 +553,8 @@ extern "C" int xtb_swiglu(const void* h_bf16, void* out_bf16, int64_t M, int I, 
   XTB_ENSURE_CTX(h_bf16);
   if (M == 0) return XTB_OK;
   const int64_t n = M * (I / 8);
-  swiglu_kernel<<<(unsigned)((n + 255) / 256), 256, 0, as_stream(stream)>>>(static_cast<const uint4*>(h_bf16),
-                                                                           static_cast<uint4*>(out_bf16), M, I / 8);
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(swiglu_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, as_stream(stream), false,
+             static_cast<const uint4*>(h_bf16), static_cast<uint4*>(out_bf16), M, I / 8);
   return XTB_OK;
 }
 
@@ -587,14 +571,8 @@ static int swiglu_bwd_impl(const char* entry, const void* grad_out_bf16, const v
   const auto* go = static_cast<const uint4*>(grad_out_bf16);
   const auto* h = static_cast<const uint4*>(h_bf16);
   auto* gh = static_cast<uint4*>(grad_h_bf16);
-  if (act_out_bf16) {
-    XTB_CUDA(launch_pdl(swiglu_bwd_kernel<true>, grid, dim3(256), 0, as_stream(stream), go, h, gh, M, I8, inv_I8,
-                        static_cast<uint4*>(act_out_bf16)));
-  } else {
-    XTB_CUDA(launch_pdl(swiglu_bwd_kernel<false>, grid, dim3(256), 0, as_stream(stream), go, h, gh, M, I8, inv_I8,
-                        static_cast<uint4*>(nullptr)));
-  }
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(act_out_bf16 ? swiglu_bwd_kernel<true> : swiglu_bwd_kernel<false>, grid, dim3(256), 0, as_stream(stream),
+             true, go, h, gh, M, I8, inv_I8, static_cast<uint4*>(act_out_bf16));
   return XTB_OK;
 }
 

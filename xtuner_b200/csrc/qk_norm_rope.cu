@@ -259,19 +259,13 @@ extern "C" int xtb_qk_norm_rope(const void* q_bf16, int64_t q_stride_t, int64_t 
   const QkOperands in{static_cast<const __nv_bfloat16*>(q_bf16), static_cast<const __nv_bfloat16*>(k_bf16), q_stride_t,
                       q_stride_h, k_stride_t, k_stride_h, Hq, Hkv};
   const dim3 grid((unsigned)((T + kQkTokens - 1) / kQkTokens));
-#define XTB_QKF(DD, NORM)                                                                                             \
-  XTB_CUDA(launch_pdl(qk_norm_rope_kernel<DD, NORM>, grid, dim3(256), 0, st, in,                                      \
-                      static_cast<const __nv_bfloat16*>(cos_bf16), static_cast<const __nv_bfloat16*>(sin_bf16), w_q_f32, \
-                      w_k_f32, static_cast<__nv_bfloat16*>(out_q_bf16), static_cast<__nv_bfloat16*>(out_k_bf16), rstd_q,  \
-                      rstd_k, T, eps))
   const bool norm = w_q_f32 != nullptr;
-  switch (D) {
-    case 64: if (norm) XTB_QKF(64, true); else XTB_QKF(64, false); break;
-    case 128: if (norm) XTB_QKF(128, true); else XTB_QKF(128, false); break;
-    default: if (norm) XTB_QKF(256, true); else XTB_QKF(256, false); break;
-  }
-#undef XTB_QKF
-  XTB_LAUNCH_OK();
+  auto* kernel = D == 64    ? (norm ? qk_norm_rope_kernel<64, true> : qk_norm_rope_kernel<64, false>)
+                 : D == 128 ? (norm ? qk_norm_rope_kernel<128, true> : qk_norm_rope_kernel<128, false>)
+                            : (norm ? qk_norm_rope_kernel<256, true> : qk_norm_rope_kernel<256, false>);
+  XTB_LAUNCH(kernel, grid, dim3(256), 0, st, true, in, static_cast<const __nv_bfloat16*>(cos_bf16),
+             static_cast<const __nv_bfloat16*>(sin_bf16), w_q_f32, w_k_f32, static_cast<__nv_bfloat16*>(out_q_bf16),
+             static_cast<__nv_bfloat16*>(out_k_bf16), rstd_q, rstd_k, T, eps);
   return XTB_OK;
 }
 
@@ -306,25 +300,18 @@ extern "C" int xtb_qk_norm_rope_bwd(const void* g_q_bf16, int64_t g_q_stride_t, 
                       q_stride_h, k_stride_t, k_stride_h, Hq, Hkv};
   const int blocks = T ? qk_bwd_blocks(T) : 0;  // T = 0: no launch; the reduce over zero partial rows writes dw = 0
   float* partial = dw ? static_cast<float*>(workspace) : nullptr;
-#define XTB_QKB(DD, NORM)                                                                                             \
-  XTB_CUDA(launch_pdl(qk_norm_rope_bwd_kernel<DD, NORM>, dim3(blocks), dim3(256), 0, st, gg, in,                      \
-                      static_cast<const __nv_bfloat16*>(cos_bf16), static_cast<const __nv_bfloat16*>(sin_bf16), w_q_f32, \
-                      w_k_f32, rstd_q, rstd_k, static_cast<__nv_bfloat16*>(dx_q_bf16),                                \
-                      static_cast<__nv_bfloat16*>(dx_k_bf16), partial, T))
   const bool norm = w_q_f32 != nullptr;
   if (T > 0) {
-    switch (D) {
-      case 64: if (norm) XTB_QKB(64, true); else XTB_QKB(64, false); break;
-      case 128: if (norm) XTB_QKB(128, true); else XTB_QKB(128, false); break;
-      default: if (norm) XTB_QKB(256, true); else XTB_QKB(256, false); break;
-    }
-    XTB_LAUNCH_OK();
+    auto* kernel = D == 64    ? (norm ? qk_norm_rope_bwd_kernel<64, true> : qk_norm_rope_bwd_kernel<64, false>)
+                   : D == 128 ? (norm ? qk_norm_rope_bwd_kernel<128, true> : qk_norm_rope_bwd_kernel<128, false>)
+                              : (norm ? qk_norm_rope_bwd_kernel<256, true> : qk_norm_rope_bwd_kernel<256, false>);
+    XTB_LAUNCH(kernel, dim3(blocks), dim3(256), 0, st, true, gg, in, static_cast<const __nv_bfloat16*>(cos_bf16),
+               static_cast<const __nv_bfloat16*>(sin_bf16), w_q_f32, w_k_f32, rstd_q, rstd_k,
+               static_cast<__nv_bfloat16*>(dx_q_bf16), static_cast<__nv_bfloat16*>(dx_k_bf16), partial, T);
   }
-#undef XTB_QKB
   if (dw) {
-    XTB_CUDA(launch_pdl(reduce_partial_rows_kernel<32>, dim3((2 * D + 31) / 32), dim3(1024), 0, st, (const float*)partial,
-                        dw, blocks, (int64_t)2 * D));
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(reduce_partial_rows_kernel<32>, dim3((2 * D + 31) / 32), dim3(1024), 0, st, true, (const float*)partial,
+               dw, blocks, (int64_t)2 * D);
   }
   return XTB_OK;
 }

@@ -705,27 +705,13 @@ extern "C" int xtb_gate_logits(const void* x_bf16, const float* w_f32, const flo
   const size_t w_smem = (size_t)E * H * sizeof(float);
   if (E <= 16 && H % 256 == 0 && w_smem <= 200 * 1024) {
     const int blocks = min(sm_count(), (T + 63) / 64);
-    if (E <= 8) {
-      static bool attr8 = false;
-      if (!attr8) {
-        XTB_CUDA(cudaFuncSetAttribute(gate_logits_small_kernel<8, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        attr8 = true;
-      }
-      XTB_CUDA(launch_pdl(gate_logits_small_kernel<8, 4>, dim3(blocks), dim3(512), w_smem, st, x, w_f32, bias_f32, logits, T, H, E));
-    } else {
-      static bool attr16 = false;
-      if (!attr16) {
-        XTB_CUDA(cudaFuncSetAttribute(gate_logits_small_kernel<16, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        attr16 = true;
-      }
-      XTB_CUDA(launch_pdl(gate_logits_small_kernel<16, 2>, dim3(blocks), dim3(512), w_smem, st, x, w_f32, bias_f32, logits, T, H, E));
-    }
-    XTB_LAUNCH_OK();
+    auto* kernel = E <= 8 ? gate_logits_small_kernel<8, 4> : gate_logits_small_kernel<16, 2>;
+    XTB_LAUNCH(kernel, dim3(blocks), dim3(512), w_smem, st, true, x, w_f32, bias_f32, logits, T, H, E);
   } else {
     dim3 grid((E + 63) / 64, (T + 63) / 64);
     // A = x [T,H] (sam=H, sak=1), B(k,n) = w[n,k] (sbk=1, sbn=H)
-    sgemm_strided_kernel<__nv_bfloat16, float><<<grid, 256, 0, st>>>(x, H, 1, w_f32, 1, H, logits, E, 1, bias_f32, T, E, H);
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(sgemm_strided_kernel<__nv_bfloat16, float>, grid, dim3(256), 0, st, false, x, H, 1, w_f32, 1, H, logits, E,
+               1, bias_f32, T, E, H);
   }
   return XTB_OK;
 }
@@ -764,34 +750,25 @@ extern "C" int xtb_gate_logits_bwd(const float* grad_logits, const void* x_bf16,
     float* partial = static_cast<float*>(workspace);
     const int cap = E <= 8 ? 512 : 256;  // threads: one per 4 columns, bounded by the kernels' launch bounds
     const int threads = (H / 4 >= cap) ? cap : ((H / 4 + 31) / 32) * 32;
-    if (E <= 8) {
-      XTB_CUDA(launch_pdl(gate_bwd_small_kernel<8>, dim3(blocks), dim3(threads), (size_t)tpb * 8 * sizeof(float), st, grad_logits, x, w_f32,
-                                                                                        partial, gx, T, H, E, tpb));
-    } else {
-      XTB_CUDA(launch_pdl(gate_bwd_small_kernel<16>, dim3(blocks), dim3(threads), (size_t)tpb * 16 * sizeof(float), st, grad_logits, x, w_f32,
-                                                                                          partial, gx, T, H, E, tpb));
-    }
-    XTB_LAUNCH_OK();
+    const int ew = E <= 8 ? 8 : 16;  // logits per token the kernel holds
+    XTB_LAUNCH(ew == 8 ? gate_bwd_small_kernel<8> : gate_bwd_small_kernel<16>, dim3(blocks), dim3(threads),
+               (size_t)tpb * ew * sizeof(float), st, true, grad_logits, x, w_f32, partial, gx, T, H, E, tpb);
     const int64_t n = (int64_t)E * H;
-    XTB_CUDA(launch_pdl(reduce_partial_rows_kernel<8>, dim3((unsigned)((n + 31) / 32)), dim3(256), 0, st, (const float*)partial, grad_w,
-                      blocks, n));
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(reduce_partial_rows_kernel<8>, dim3((unsigned)((n + 31) / 32)), dim3(256), 0, st, true,
+               (const float*)partial, grad_w, blocks, n);
   } else {
     // grad_x[T,H] = gl[T,E] @ w[E,H]:  A = gl (sam=E, sak=1), B(k=e, n=h) = w[e,h] (sbk=H, sbn=1)
     dim3 g1((H + 63) / 64, (T + 63) / 64);
-    sgemm_strided_kernel<float, __nv_bfloat16><<<g1, 256, 0, st>>>(grad_logits, E, 1, w_f32, H, 1, gx, H, 1, nullptr,
-                                                                   T, H, E);
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(sgemm_strided_kernel<float, __nv_bfloat16>, g1, dim3(256), 0, st, false, grad_logits, E, 1, w_f32, H, 1, gx,
+               H, 1, nullptr, T, H, E);
     // grad_w[e,h] = sum_t gl[t,e] x[t,h]:  A(m=h, k=t) = x[t,h] (sam=1, sak=H), B(k=t, n=e) = gl[t,e]
     // (sbk=E, sbn=1), C(m=h, n=e) -> grad_w[e*H + h] (scm=1, scn=H)
     dim3 g2((E + 63) / 64, (H + 63) / 64);
-    sgemm_strided_kernel<__nv_bfloat16, float><<<g2, 256, 0, st>>>(x, 1, H, grad_logits, E, 1, grad_w, 1, H, nullptr,
-                                                                   H, E, T);
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(sgemm_strided_kernel<__nv_bfloat16, float>, g2, dim3(256), 0, st, false, x, 1, H, grad_logits, E, 1, grad_w,
+               1, H, nullptr, H, E, T);
   }
   if (grad_bias) {
-    colsum_kernel<<<E, 256, 0, st>>>(grad_logits, grad_bias, T, E);
-    XTB_LAUNCH_OK();
+    XTB_LAUNCH(colsum_kernel, dim3(E), dim3(256), 0, st, false, grad_logits, grad_bias, T, E);
   }
   return XTB_OK;
 }
@@ -816,11 +793,10 @@ static int launch_router_greedy(const float* logits, int T, int E, int K, int sc
   } else {
     XTB_CUDA(cudaMemsetAsync(tpe, 0, sizeof(int64_t) * E, st));
   }
-  XTB_CUDA(launch_pdl(replay_ids ? router_greedy_kernel<LPT, VPL, true> : router_greedy_kernel<LPT, VPL>, dim3(blocks),
-                      dim3(kThreads), smem, st, logits, T, E, K, scoring, norm, scaling, rw, tw, ids, ids32,
-                      reinterpret_cast<unsigned long long*>(tpe), counts, estart, ticket, n_chunks_of(T), replay_ids,
-                      replay_stride));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(replay_ids ? router_greedy_kernel<LPT, VPL, true> : router_greedy_kernel<LPT, VPL>, dim3(blocks),
+             dim3(kThreads), smem, st, true, logits, T, E, K, scoring, norm, scaling, rw, tw, ids, ids32,
+             reinterpret_cast<unsigned long long*>(tpe), counts, estart, ticket, n_chunks_of(T), replay_ids,
+             replay_stride);
   return XTB_OK;
 }
 
@@ -830,9 +806,8 @@ static int launch_router_greedy_bwd(const float* rw, const float* tw, const int6
                                     int norm, float scaling, float* gl, cudaStream_t st) {
   const int tokens_per_block = 256 / LPT;
   const int blocks = (T + tokens_per_block - 1) / tokens_per_block;
-  XTB_CUDA(launch_pdl(router_greedy_bwd_kernel<LPT, VPL>, dim3(blocks), dim3(256), 0, st, rw, tw, ids, g_tw, g_rw, g_direct, T, E, K, scoring,
-                                                            norm, scaling, gl));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(router_greedy_bwd_kernel<LPT, VPL>, dim3(blocks), dim3(256), 0, st, true, rw, tw, ids, g_tw, g_rw, g_direct,
+             T, E, K, scoring, norm, scaling, gl);
   return XTB_OK;
 }
 
@@ -852,9 +827,8 @@ static int launch_router_noaux_bwd(const float* logits, const float* bias, const
                                    int n_group, int topk_group, int norm, float scaling, float* gl, cudaStream_t st) {
   const int tokens_per_block = 256 / LPT;
   const int blocks = (T + tokens_per_block - 1) / tokens_per_block;
-  XTB_CUDA(launch_pdl(router_noaux_bwd_kernel<LPT, VPL>, dim3(blocks), dim3(256), 0, st, logits, bias, rw, tw, ids,
-                      g_tw, g_rw, T, E, K, n_group, topk_group, norm, scaling, gl));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(router_noaux_bwd_kernel<LPT, VPL>, dim3(blocks), dim3(256), 0, st, true, logits, bias, rw, tw, ids,
+             g_tw, g_rw, T, E, K, n_group, topk_group, norm, scaling, gl);
   return XTB_OK;
 }
 
@@ -958,21 +932,19 @@ static int router_noaux_impl(const float* logits, const float* e_score_correctio
   XTB_CUDA(cudaMemsetAsync(tokens_per_expert_f32, 0, sizeof(float) * E, st));
   if (T == 0) return XTB_OK;
   const int blocks = (T + 7) / 8;
-#define XTB_NOAUX(V)                                                                                                  \
-  XTB_CUDA(launch_pdl(replay_ids ? router_noaux_kernel<V, true> : router_noaux_kernel<V>, dim3(blocks), dim3(256),    \
-                      E * sizeof(int), st, logits, e_score_correction_bias, T, E, K, n_group, topk_group,             \
-                      norm_topk_prob, scaling, router_weights, topk_weights, topk_ids, topk_ids_i32,                  \
-                      tokens_per_expert_f32, replay_ids, replay_stride))
+  const bool replay = replay_ids != nullptr;
+  decltype(&router_noaux_kernel<1>) kernel;
   switch (E / 32) {
-    case 1: XTB_NOAUX(1); break;
-    case 2: XTB_NOAUX(2); break;
-    case 4: XTB_NOAUX(4); break;
-    case 8: XTB_NOAUX(8); break;
-    case 16: XTB_NOAUX(16); break;
+    case 1: kernel = replay ? router_noaux_kernel<1, true> : router_noaux_kernel<1>; break;
+    case 2: kernel = replay ? router_noaux_kernel<2, true> : router_noaux_kernel<2>; break;
+    case 4: kernel = replay ? router_noaux_kernel<4, true> : router_noaux_kernel<4>; break;
+    case 8: kernel = replay ? router_noaux_kernel<8, true> : router_noaux_kernel<8>; break;
+    case 16: kernel = replay ? router_noaux_kernel<16, true> : router_noaux_kernel<16>; break;
     default: return fail(XTB_ERR_INVALID, "xtb_router_noaux: E/32=%d unsupported (1,2,4,8,16)", E / 32);
   }
-#undef XTB_NOAUX
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(kernel, dim3(blocks), dim3(256), E * sizeof(int), st, true, logits, e_score_correction_bias, T, E, K, n_group,
+             topk_group, norm_topk_prob, scaling, router_weights, topk_weights, topk_ids, topk_ids_i32,
+             tokens_per_expert_f32, replay_ids, replay_stride);
   return XTB_OK;
 }
 
@@ -1054,13 +1026,11 @@ extern "C" int xtb_router_gate_bwd(const float* router_weights, const float* top
   const auto* x = static_cast<const __nv_bfloat16*>(x_bf16);
   auto* gx = static_cast<__nv_bfloat16*>(grad_x_bf16);
   const size_t smem = (size_t)tpb * 8 * sizeof(float);
-  XTB_CUDA(launch_pdl(router_gate_bwd_kernel, dim3(blocks), dim3(threads), smem, st, router_weights, topk_weights, topk_ids,
-                      grad_topk_weights, grad_router_weights, grad_logits_direct, K, scoring, norm_topk_prob, scaling, x, w_f32,
-                      partial, gx, T, H, E, tpb));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(router_gate_bwd_kernel, dim3(blocks), dim3(threads), smem, st, true, router_weights, topk_weights, topk_ids,
+             grad_topk_weights, grad_router_weights, grad_logits_direct, K, scoring, norm_topk_prob, scaling, x, w_f32,
+             partial, gx, T, H, E, tpb);
   const int64_t n = (int64_t)E * H;
-  XTB_CUDA(launch_pdl(reduce_partial_rows_kernel<8>, dim3((unsigned)((n + 31) / 32)), dim3(256), 0, st, (const float*)partial, grad_w,
-                      blocks, n));
-  XTB_LAUNCH_OK();
+  XTB_LAUNCH(reduce_partial_rows_kernel<8>, dim3((unsigned)((n + 31) / 32)), dim3(256), 0, st, true, (const float*)partial, grad_w,
+             blocks, n);
   return XTB_OK;
 }
